@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — the video->text prefill path of VideoLLaMA2-7B (16 frames @336, 256-token prompt) on B200.
+"""bench.py — the video->text prefill path of VideoLLaMA2-7B (16 frames @336, 256-token prompt) on H100.
 
-  python bench.py --gpus N --steps K --warmup W            our arm (libvl2 sm_100a kernels)
+  python bench.py --gpus N --steps K --warmup W            our arm (libvl2 sm_90a kernels)
   python bench.py --impl reference ...                      the reference's own PyTorch-CPU path (oracle port), rank 0 only
 
 A "step" is one pass of the hot path over one video: pixels + prompt ids -> ViT -> STC connector -> splice -> decoder
@@ -10,7 +10,8 @@ prefill -> last-position logits.  `value` = prefill tokens/s of the WHOLE job wi
 `e2e` = the same through the public API (model.generate(..., max_new_tokens=1)) from pinned HOST buffers with the
 H2D copy of the frames and the D2H read of the result inside the timed region.  `frame_parallel` reports the
 frame-sharded ViT + NCCL all-gather stage (strong scaling of one video's vision stage) when N > 1.
-One JSON line on stdout (rank 0).  Nothing here reads /root/reference.
+One JSON line on stdout (rank 0).  `--dump-outputs DIR` also writes the last timed step's logits as DIR/logits.npy
+(float32; the inputs are seeded, so two builds can be compared output for output).
 """
 from __future__ import annotations
 
@@ -26,7 +27,7 @@ import time
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-METRIC = "video-frames/sec + prefill tokens/sec (VideoLLaMA2-7B, 16f@336) at 1/2/4/8 B200"
+METRIC = "video-frames/sec + prefill tokens/sec (VideoLLaMA2-7B, 16f@336) at 1/2/4/8 H100"
 FRAMES, PROMPT = 16, 256
 WORKLOAD = ("VideoLLaMA2-7B ({model}) 16 frames@{img} + 256-token prompt -> S={S} prefill, last-position logits; "
             "one video per GPU")
@@ -38,11 +39,12 @@ def peaks():
         d = json.load(open(p))
         return {"bf16_burst": d["bf16_tflops"], "bf16_sustained": d["bf16_tflops_sustained"], "hbm_gbs": d["hbm_gbs"],
                 "src": "measured"}
-    return {"bf16_burst": 1590.0, "bf16_sustained": 1400.0, "hbm_gbs": 6650.0, "src": "fallback"}
+    # H100 SXM data sheet (dense bf16, HBM3), not a measurement
+    return {"bf16_burst": 989.0, "bf16_sustained": 989.0, "hbm_gbs": 3350.0, "src": "H100 SXM data sheet"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -415,6 +417,8 @@ def main():
     ap.add_argument("--gpu-rng-weights", action="store_true",
                     help="random weights from the device RNG (fast start-up; the output can then not be parity-checked)")
     ap.add_argument("--no-kernel-profile", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs (last-position logits) as DIR/<name>.npy, float32")
     ap.add_argument("--decode-tokens", type=int, default=16, help="extra (untimed-region) KV-cache decode measurement; 0 = skip")
     ap.add_argument("--no-graphs", action="store_true", help="launch every kernel eagerly instead of replaying CUDA graphs")
     ap.add_argument("--profile-one-step", action="store_true",
@@ -492,9 +496,12 @@ def main():
     px_dev = px_host.to(dev)
     mask = torch.ones_like(ids_host, dtype=torch.bool)
 
+    last = {}
+
     def step_resident():
         _, _, _, emb, _ = model.prepare_inputs_labels_for_multimodal(ids_host, mask, None, None, [(px_dev, "video")])
         logits, _ = model.get_model().decoder.prefill(emb[0], all_logits=False)
+        last["logits"] = logits
         return logits
 
     def step_e2e():
@@ -548,6 +555,10 @@ def main():
         sampler.start()
     ms_step, t0, t1 = timed(step_resident, args.steps)
     clocks = sampler.stop(t0, t1) if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "logits.npy"), last["logits"].float().cpu().numpy())
 
     for _ in range(2):
         step_e2e()
@@ -585,7 +596,7 @@ def main():
             ms_tok = ms_tok_dev                                  # quota-throttled host, so the device-timed figure is the headline
             w_bytes = sum(t.numel() * t.element_size() for L in model.get_model().decoder.layers for t in L.values())
             w_bytes += model.get_model().decoder.w["lm_head"].numel() * 2
-            hbm = float(peaks().get("hbm_gbs") or 6500.0)
+            hbm = float(peaks().get("hbm_gbs") or 3350.0)
             decode = {"new_tokens": got, "ms_per_token": ms_tok, "ms_per_token_device_timed": ms_tok_dev,
                       "ms_per_token_generate_wall": ms_wall if ms_wall > 0 else None,
                       "tok_per_s": 1e3 / ms_tok if ms_tok > 0 else None,
@@ -615,7 +626,7 @@ def main():
         prep = {"input": f"{FRAMES} x 1080x1920x3 uint8 (pad to square, Pillow-exact bicubic to {IMG}, normalise, bf16)",
                 "ms_resident": ms_prep_dev, "ms_from_pinned_host": ms_prep_e2e, "frames_per_s": FRAMES / (ms_prep_dev * 1e-3),
                 "algorithmic_bytes": int(algo), "achieved_gbps": algo / ms_prep_dev / 1e6,
-                "frac_of_hbm": algo / ms_prep_dev / 1e6 / float(peaks().get("hbm_gbs") or 6500.0),
+                "frac_of_hbm": algo / ms_prep_dev / 1e6 / float(peaks().get("hbm_gbs") or 3350.0),
                 "h2d_bytes": int(in_bytes)}
         del raw_dev
 
@@ -638,7 +649,7 @@ def main():
     t_vis = statistics.median(s[1] for s in st)      # ViT + STC + splice (encode_images_or_videos inside)
     t_llm = statistics.median(s[2] for s in st)
 
-    # dominant-kernel roofline: every tcgen05 GEMM launch of one step bracketed by CUDA events on the launch stream
+    # dominant-kernel roofline: every GEMM launch of one step bracketed by CUDA events on the launch stream
     roof = None
     model.enable_cuda_graphs(False)      # per-kernel event timing needs eager launches
     l0 = ops.launch_count()
@@ -683,7 +694,7 @@ def main():
             else:
                 traffic_src = "profiles/r02_gemm_dram_traffic.json is from another build (digest mismatch): not reported"
         ach = g_fl / (g_ms * 1e-3) / 1e12
-        roof = {"bound": "tensor", "kernel": "gemm_bf16_tcgen05_kernel", "achieved": ach, "peak": pk["bf16_sustained"],
+        roof = {"bound": "tensor", "kernel": "gemm_bf16_wgmma_kernel", "achieved": ach, "peak": pk["bf16_sustained"],
                 "unit": "TFLOP/s", "frac": ach / pk["bf16_sustained"], "traffic": traffic, "traffic_src": traffic_src, "launches": len(recs),
                 "avg_launch_ms": g_ms / max(1, len(recs)), "flops_per_launch": g_fl / max(1, len(recs)),
                 "gemm_ms_per_step": g_ms, "gemm_share_of_step": g_ms / ms_step, "peak_src": pk["src"] + " sustained",
@@ -770,7 +781,7 @@ def main():
                        f"deterministic synthetic checkpoint (host RNG, seed {presets.SYNTH_SEED}; {weights_s:.0f}s to generate + load)",
                        "parallelism": f"replicas x{world} (+ frame-sharded ViT reported separately)",
                        "cuda_graphs": not args.no_graphs,
-                       "l2": "weights (16 GB) >> L2 (126 MB): every step streams them from HBM; no explicit flush",
+                       "l2": "weights (16 GB) >> L2 (50 MB): every step streams them from HBM; no explicit flush",
                        "flops_per_step": fl["total"]},
             "frames_per_s": world * FRAMES / (t_vis * 1e-3), "vit_frames_per_s": world * FRAMES / (t_vit * 1e-3),
             "llm_prefill_tok_per_s": world * S / (t_llm * 1e-3),

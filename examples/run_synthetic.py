@@ -3,7 +3,7 @@ decoded uint8 frames -> device preprocessing -> tower -> connector -> splice -> 
 
     python examples/run_synthetic.py [--model mistral7b|qwen2_7b|qwen2_7b_v21] [--frames 16] [--new-tokens 32]
 
-Needs one B200 and ~20 GB of HBM (the 7B decoder in bf16).  The token ids are meaningless (random weights); the point is
+Needs one H100 and ~20 GB of HBM (the 7B decoder in bf16).  The token ids are meaningless (random weights); the point is
 the call sequence a user of the reference's `mm_infer` would make, and the timings."""
 import argparse
 import os

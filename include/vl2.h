@@ -1,5 +1,5 @@
 /*
- * vl2.h — C-ABI of libvl2.so, the B200 (sm_100a) kernel library behind the VideoLLaMA2 video->text prefill path.
+ * vl2.h — C-ABI of libvl2.so, the H100 (sm_90a) kernel library behind the VideoLLaMA2 video->text prefill path.
  *
  * The reference (DAMO-NLP-SG/VideoLLaMA2) is pure Python on top of HF transformers / timm / torch; it has no FFI.
  * Each entry point below therefore replaces a *library call site* of the reference hot path; the citation after
@@ -12,7 +12,7 @@
  *  - `stream` is a cudaStream_t passed as void*.  Calls enqueue work and return; they never synchronise, never
  *    allocate device memory, and are CUDA-graph capturable.
  *  - Every call returns 0 on success or a negative VL2_E_* code; vl2_last_error() gives a thread-local message.
- *  - There is no CPU fallback: on a machine without an sm_100 device the calls fail with VL2_E_CUDA.
+ *  - There is no CPU fallback: on a machine without an sm_90 device the calls fail with VL2_E_CUDA.
  */
 #ifndef VL2_H_
 #define VL2_H_
@@ -62,7 +62,7 @@ int64_t vl2_launch_count(void);
 int vl2_set_pdl(int mode);
 
 /* ------------------------------------------------------------------------------------------------------------
- * Dense bf16 GEMM on tcgen05 tensor cores:  C[M,Nout] = epi( A[M,K] * W[N,K]^T ).
+ * Dense bf16 GEMM on the Hopper tensor cores (wgmma):  C[M,Nout] = epi( A[M,K] * W[N,K]^T ).
  *   epi(acc) = act( acc * row_scale[m] + bias[n] ) + residual[m,n]        (each term optional)
  *   VL2_ACT_SWIGLU: W rows interleave gate/up (row 2j = gate_j, row 2j+1 = up_j); Nout = N/2; residual unsupported.
  * Replaces nn.Linear / 1x1 nn.Conv2d / (after im2col) nn.Conv2d and nn.Conv3d call sites:
@@ -82,7 +82,7 @@ typedef struct vl2_gemm_args {
   int32_t act;
   int32_t out_f32;
   int32_t reserved; /* 0 = choose the tile by the library's cost model; 64..256 (step 32) forces a single-CTA tile width,
-                       1000 + (128..256) forces the cta_group::2 pair kernel (tests) */
+                       1000 + (128..256) forces the two-CTA cluster kernel (256-row tile, B multicast) (tests) */
   /* Fused compute + collective (frame-parallel ViT, SURVEY.md §8e): every output vector of C is ALSO stored at the same
    * element offset into up to 8 peer buffers (other GPUs' symmetric memory mapped over NVLink), or once to an NVSwitch
    * multicast address (multimem.st) when mc_out != NULL — the all-gather of visual tokens happens inside the epilogue
@@ -131,8 +131,7 @@ typedef struct vl2_gemm_args {
    * The TMA producer gathers each k-block (one tap x 64 channels) of 8 output lines straight from x with ONE box of a 5-D
    * tensor map over x viewed as [T, H/2, 2, W/2, 2C] (out-of-bounds = the zero padding): no im2col matrix exists.
    * Up to 16 x 16 output positions per time step; odd H / W only with conv_pad = 0.  lda is ignored.  bias + activation
-   * epilogues only.  reserved4: 0; test hook 1 = use the general epilogue where the lean (TMA-store) one would be
-   * picked (both are parity-tested against each other). */
+   * epilogues only.  reserved4: must be 0. */
   int32_t conv_C, conv_T, conv_H, conv_W, conv_pad, reserved4;
   /* RoPE in the epilogue of the fused QKV projection (HF:mistral/modeling_mistral.py:51-82 apply_rotary_pos_emb): output
    * columns [0, rope_cols) are q and k heads of width rope_D whose weight rows were permuted at load so that the rotation
@@ -151,8 +150,8 @@ int vl2_gemm_bf16(const vl2_gemm_args* args, void* stream);
  * warp's first 64-column span (start, residual staged, accumulator chunk loaded, first / second half computed, stored).
  * host_out128: 128 values.  Synchronises the device. */
 int vl2_debug_gemm_trace(long long* host_out128);
-/* Planning only, no device work: out6 = {tile width BN, 1 if the 256-row cta_group::2 tile is used, number of tiles,
- * CTAs (or CTA pairs) the persistent grid runs, rounds = ceil(tiles / that), SM count assumed (148 without a device)}. */
+/* Planning only, no device work: out6 = {tile width BN, 1 if the 256-row two-CTA tile is used, number of tiles,
+ * CTAs (or CTA pairs) the persistent grid runs, rounds = ceil(tiles / that), SM count assumed (132, an H100 SXM, without a device)}. */
 int vl2_gemm_plan(int M, int N, int K, int with_splitk_ws, int32_t* out6);
 
 /* Skinny GEMM (M <= 32 rows, HBM-bound weight streaming): C[M,N] = act(A[M,K] W[N,K]^T + bias).
@@ -171,7 +170,7 @@ int vl2_gemv_bf16(const void* x, const void* W, const float* bias, const void* r
                   int out_f32, int N, int K, int act, float rms_eps, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
- * Fused attention (FlashAttention-style, tcgen05 QK^T / PV with TMEM accumulators, TMA-staged K/V).
+ * Fused attention (FlashAttention-style, wgmma QK^T / PV with register accumulators, TMA-staged K/V).
  *   q: bf16 [B*S, ldq] with head h at columns [q_off + h*D, +D)   (likewise k, v with kv head h / (Hq/Hkv))
  *   out: bf16 [B*S, ldo], head h at columns [h*D, +D).  softmax scale applied to logits in fp32.
  * causal = 0: HF:clip/modeling_clip.py:282-336 (CLIPAttention, 16 heads x 64).
@@ -191,16 +190,10 @@ typedef struct vl2_attn_args {
   int32_t reserved;
 } vl2_attn_args;
 int vl2_attention(const vl2_attn_args* args, void* stream);
-/* Debug aid: with args->reserved == 777 one softmax thread of CTA (0,0,0) accumulates the cycles it spends in each
+/* Debug aid: with args->reserved == 777 consumer thread 0 of CTA (0,0,0) accumulates the cycles it spends in each
  * phase of the key-tile loop; this call synchronises the device and copies the 16 counters to host memory
- * ([0] wait S, [1] TMEM load, [2] mask+max+exchange, [3] wait PV / rescale, [4] exp2+pack+st.shared, [5] fence+arrive,
- *  [6] item epilogue, [7] key tiles traced, [8] work items traced, [9] cycles of the CTA's whole item loop);
- * reserved == 778 traces every work item of the persistent CTA 0 instead of its first (cold) one. */
+ * ([0] wait for K, [1] Q K^T + softmax, [2] wait for V + P V, [7] key tiles traced, [8] work items traced). */
 int vl2_debug_attn_trace(long long* host_out16);
-/* Debug aid: with args->reserved == 779 the softmax thread, the MMA-issuing thread and the two TMA producer lanes of the
- * persistent CTA 0 stamp clock64() at every hand-over of its second work item (slot map: csrc/attn_tcgen05.cu,
- * g_attn_tl); this call synchronises the device and copies the 320 stamps to host memory (tools/attn_trace.py). */
-int vl2_debug_attn_timeline(long long* host_out320);
 
 /* Hint: pull [ptr, ptr + bytes) into L2 (cp.async.bulk.prefetch.L2 in 16 KB pieces; returns immediately).  The decode graph
  * forks this next to the latency-bound attention phase so the o_proj / gate-up GEMVs start from L2-resident weights. */
@@ -319,7 +312,7 @@ int vl2_preprocess_frames(const vl2_preprocess_args* args, void* stream);
  * pixels bf16 [F,3,H,W]; weight bf16 [C, Kpad] = patch_embedding.weight flattened (c, i, j)-major and zero-padded from
  * 3*P*P to Kpad (multiple of 64, <= 640); pos bf16 [np (+1), C]; out bf16 [F*(np (+1)), C].  The A operand is gathered
  * from the frames by the kernel (LDG -> 128B-swizzled shared memory); no im2col matrix exists.  A 128-patch row block is
- * split along C over a thread-block cluster of up to 4 CTAs that keep their accumulators in TMEM and exchange the
+ * split along C over a thread-block cluster of up to 8 CTAs that keep their accumulators in registers and exchange the
  * LayerNorm statistics through distributed shared memory: nothing un-normalised leaves the SM (`scratch` is unused).
  * ---------------------------------------------------------------------------------------------------------- */
 typedef struct vl2_patch_embed_args {
@@ -360,7 +353,7 @@ typedef struct vl2_tp_allreduce_args {
   int32_t rank, world, S, H;
   uint32_t epoch;
   uint32_t inswitch_reduce; /* 1: reduce inside the NVSwitch (multimem.ld_reduce; needs *_mc).  Off by default: measured on
-                               B200 the switch does not round bf16 sums to nearest (1-ulp differences on ~19 % of the
+                               the switch does not round bf16 sums to nearest (1-ulp differences on ~19 % of the
                                elements), so the default reduces with peer loads (exact fp32 accumulation) and uses the
                                switch for the broadcast only */
 } vl2_tp_allreduce_args;

@@ -15,6 +15,7 @@ from . import preprocess_ref as P
 from . import ref_loader
 
 OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden", "preprocess.pt")
+OUT_HD = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden", "preprocess_hd.pt")
 
 CASES = [   # (name, T, H, W, size, kind, aspect_ratio)
     ("landscape_pad_clip", 3, 90, 160, 56, "clip", "pad"),
@@ -50,6 +51,17 @@ def reference_pipeline(mm_utils, frames, size, kind, aspect_ratio):
     return u8, np.ascontiguousarray(x.transpose(0, 3, 1, 2))
 
 
+def save_deflated(obj, path):
+    """torch.save, then the archive's members deflated (torch.load reads either form): the uint8 frames are mostly smooth."""
+    import io
+    import zipfile
+    buf = io.BytesIO()
+    torch.save(obj, buf)
+    with zipfile.ZipFile(io.BytesIO(buf.getvalue())) as zi, zipfile.ZipFile(path, "w", zipfile.ZIP_DEFLATED, compresslevel=9) as zo:
+        for info in zi.infolist():
+            zo.writestr(info.filename, zi.read(info.filename))
+
+
 def main():
     ref_loader.load()
     mm_utils = importlib.import_module("videollama2.mm_utils")
@@ -72,8 +84,11 @@ def main():
                               "frames": torch.from_numpy(frames), "u8": torch.from_numpy(u8),
                               # float32 pixel_values only for the small cases (fixture size); u8 -> float is a 256-entry map
                               "pixel_values": torch.from_numpy(px) if size <= 70 else None}
-    torch.save(out, OUT)
-    print("wrote", OUT, os.path.getsize(OUT) // 1024, "KiB")
+    # the HD case goes to a file of its own: every committed fixture stays under 1 MB
+    hd = {"cases": {k: out["cases"].pop(k) for k in list(out["cases"]) if out["cases"][k]["H"] * out["cases"][k]["W"] >= 360 * 640}}
+    for path, obj in ((OUT, out), (OUT_HD, hd)):
+        save_deflated(obj, path)
+        print("wrote", path, os.path.getsize(path) // 1024, "KiB")
 
 
 if __name__ == "__main__":

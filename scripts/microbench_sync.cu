@@ -1,6 +1,6 @@
 // Latency of the synchronisation primitives the attention kernel's softmax warps use, measured in isolation:
 // successful mbarrier try_wait / test_wait (1 warp vs 8 warps polling the same barrier), bar.sync over 256 / 64 threads,
-// __syncwarp, st.shared + ld.shared exchange.  Build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a
+// __syncwarp, st.shared + ld.shared exchange.  Build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (sm_100a); run with `pytest -m gpu` on the B200 box")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (sm_90a, an H100); run with `pytest -m gpu`")
 
 
 @pytest.fixture(scope="session")

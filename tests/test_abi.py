@@ -115,23 +115,23 @@ def test_plain_c_consumer_links_and_validates(lib, tmp_path):
 
 def test_gemm_plan_for_the_path_shapes(lib):
     """vl2_gemm_plan is host logic only: the tile the cost model picks and how many rounds the persistent grid runs for
-    the GEMMs of config 2 (148 SMs assumed without a device).  Pins the scheduler against accidental changes."""
+    the GEMMs of config 2 (132 SMs, an H100 SXM, assumed without a device).  Pins the scheduler against accidental changes."""
     def plan(M, N, K):
         out = (ctypes.c_int32 * 6)()
         assert lib.vl2_gemm_plan(M, N, K, 0, out) == 0
         return dict(zip(("bn", "pair", "tiles", "slots", "rounds", "sms"), out))
-    gate_up = plan(1776, 28672, 4096)            # decoder gate/up: the 256 x 256 cta_group::2 tile, 784 tiles on 74 pairs
-    assert (gate_up["bn"], gate_up["pair"], gate_up["tiles"], gate_up["slots"], gate_up["rounds"]) == (256, 1, 784, 74, 11)
+    gate_up = plan(1776, 28672, 4096)            # decoder gate/up: the 256 x 256 two-CTA tile, 784 tiles on 66 pairs
+    assert (gate_up["bn"], gate_up["pair"], gate_up["tiles"], gate_up["slots"], gate_up["rounds"]) == (256, 1, 784, 66, 12)
     for M, N, K in [(1776, 6144, 4096), (1776, 4096, 4096), (1776, 4096, 14336), (9232, 3072, 1024), (9232, 4096, 1024),
                     (9232, 1024, 4096), (11664, 1152, 1152)]:
         p = plan(M, N, K)
-        assert p["pair"] == 1 and p["bn"] in (224, 256, 416) and p["sms"] == 148   # 416 = the wide 224 + 192 tile
+        assert p["pair"] == 1 and p["bn"] in (192, 224, 256) and p["sms"] == 132
         tile_m = 256
         assert p["tiles"] == -(-M // tile_m) * -(-N // p["bn"]) and p["rounds"] == -(-p["tiles"] // p["slots"])
-    o_proj, down = plan(1776, 4096, 4096), plan(1776, 4096, 14336)   # one round of wide tiles instead of two narrow ones
-    assert (o_proj["bn"], o_proj["rounds"], down["bn"], down["rounds"]) == (416, 1, 416, 1)
-    assert plan(1776, 6144, 4096)["bn"] == 224 and plan(9232, 1024, 1024)["bn"] == 256
-    small = plan(300, 520, 256)                  # a matrix narrower than a wide tile gets a narrow single-CTA tile
+    o_proj, down = plan(1776, 4096, 4096), plan(1776, 4096, 14336)   # 7 x 16 tiles: two rounds of the 66 pairs
+    assert (o_proj["bn"], o_proj["rounds"], down["bn"], down["rounds"]) == (256, 2, 256, 2)
+    assert plan(1776, 6144, 4096)["bn"] == 224 and plan(9232, 1024, 1024)["bn"] == 224
+    small = plan(300, 520, 256)                  # a small matrix gets a narrow single-CTA tile
     assert small["pair"] == 0 and small["bn"] <= 128 and small["rounds"] == 1
     out = (ctypes.c_int32 * 6)()
     assert lib.vl2_gemm_plan(0, 8, 8, 0, out) < 0

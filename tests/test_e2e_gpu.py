@@ -1,4 +1,4 @@
-"""End-to-end parity of the B200 engine against the CPU oracle (oracle/torch_ref.py, fp32 math on the same bf16-rounded
+"""End-to-end parity of the engine against the CPU oracle (oracle/torch_ref.py, fp32 math on the same bf16-rounded
 synthetic weights = "G32"), stage by stage and through the reference-shaped public API.
 
 Tolerances (SURVEY.md §8c): relL2 <= 1e-2 against the fp32 golden for a stage fed the golden's stage input

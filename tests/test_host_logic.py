@@ -1,6 +1,6 @@
 """Exact (integer) parity of the host-side token / splice logic with the reference
 (videollama2/mm_utils.py:277-302, videollama2/model/videollama2_arch.py:161-263) via the committed fixtures, and live
-against the reference functions when /root/reference exists."""
+against what the reference functions returned (tests/golden)."""
 import os
 
 import pytest
@@ -62,18 +62,20 @@ def test_splice_plan_edge_cases():
     assert m[0].all() and m[1].tolist() == [True] * 3 + [False] * 6
 
 
+def _live_gold():
+    """What the reference classes computed for these tests (oracle/make_golden_live.py -> tests/golden/live_reference.pt)."""
+    return torch.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "live_reference.pt"))
+
+
 def test_live_reference_splice_and_tokenizer():
-    from oracle import ref_loader
-    if not ref_loader.available():
-        pytest.skip("/root/reference not present")
-    import importlib
-    ref_loader.load()
-    ref_mm = importlib.import_module("videollama2.mm_utils")
     from oracle.make_golden import PROMPTS, ToyTokenizer
+    from oracle.make_golden_live import TOKENIZER_PROMPTS_EXTRA
     from videollama2_b200 import mm_utils
     tok = ToyTokenizer()
-    for p, t in PROMPTS + [("a <video> b <video> c", "<video>"), ("", "<video>")]:
-        assert mm_utils.tokenizer_multimodal_token(p, tok, t) == ref_mm.tokenizer_multimodal_token(p, tok, t)
+    gold = _live_gold()["tokenizer"]
+    assert [(p, t) for p, t, _ in gold] == PROMPTS + TOKENIZER_PROMPTS_EXTRA
+    for p, t, want in gold:
+        assert mm_utils.tokenizer_multimodal_token(p, tok, t) == want
 
 
 def test_keywords_stopping_criteria():
@@ -189,14 +191,12 @@ def test_mm_infer_matches_reference_goldens():
 
 
 def test_mm_infer_matches_live_reference():
-    from oracle import mm_infer_ref, ref_loader
-    if not ref_loader.available():
-        pytest.skip("/root/reference not present: the committed goldens cover this")
+    from oracle import mm_infer_ref
     instruct, modal, mtype, kw = mm_infer_ref.CASES[0]
-    text, call = mm_infer_ref.run_reference(instruct, modal, mtype, torch.zeros((2, 3, 4, 4)), **kw)
+    gold = _live_gold()["mm_infer"]
     case = {"instruct": instruct, "modal": modal, "model_type": mtype, "kwargs": kw}
     my_text, mine, _ = _my_mm_infer_call(case)
-    assert my_text == text and torch.equal(mine["input_ids"], mm_infer_ref.summarise(call)["input_ids"])
+    assert my_text == gold["text"] and torch.equal(mine["input_ids"], gold["input_ids"])
     import videollama2_b200
     with pytest.raises(ValueError):
         videollama2_b200.mm_infer(None, "x", mm_infer_ref.RecordingModel("videollama2"), mm_infer_ref.ToyChatTokenizer(), modal="audio")
@@ -322,28 +322,27 @@ class _DecodingToyTokenizer:
         return ["".join(self._VOCAB[int(t) - 3] for t in row if int(t) >= 3) for row in ids]
 
 
-def test_keywords_stopping_criteria_decoded_text_branch_matches_reference():
-    """mm_utils.py:332-337: the keyword may be spelled by different ids than tokenizer(keyword) produced; the decoded tail
-    (window = longest keyword, in ids) is searched too.  Compared call by call with the reference class when
-    /root/reference exists."""
-    from videollama2_b200.mm_utils import KeywordsStoppingCriteria
-    tok = _DecodingToyTokenizer()
-    prompt = torch.zeros(1, 2, dtype=torch.long)
-    ours = KeywordsStoppingCriteria(["hello"], tok, prompt)
+def keyword_cases(tok):
+    """Id sequences for the decoded-text branch of KeywordsStoppingCriteria (also fed to the reference by
+    oracle/make_golden_live.py)."""
     kw = tok("hello", add_special_tokens=False).input_ids             # ["he", "llo"]
     bang = tok("hello!", add_special_tokens=False).input_ids          # one id spelling "hello!"
     assert len(kw) == 2 and len(bang) == 1
     x, y = tok("x", add_special_tokens=False).input_ids[0], tok("y", add_special_tokens=False).input_ids[0]
-    cases = [torch.tensor([[x, y] + kw]), torch.tensor([[x, y, x] + bang]), torch.tensor([[x, y, x, y]]),
-             torch.tensor([bang]), torch.tensor([[x] + bang + [y, y, y, y]]), torch.tensor([[x, y, y] + bang + [y]]),
-             torch.tensor([[x, y] + kw, [x, y, y, y]]), torch.tensor([[x] + kw, [y] + kw])]
-    got = [ours(c, None) for c in cases]
+    return [torch.tensor([[x, y] + kw]), torch.tensor([[x, y, x] + bang]), torch.tensor([[x, y, x, y]]),
+            torch.tensor([bang]), torch.tensor([[x] + bang + [y, y, y, y]]), torch.tensor([[x, y, y] + bang + [y]]),
+            torch.tensor([[x, y] + kw, [x, y, y, y]]), torch.tensor([[x] + kw, [y] + kw])]
+
+
+def test_keywords_stopping_criteria_decoded_text_branch_matches_reference():
+    """mm_utils.py:332-337: the keyword may be spelled by different ids than tokenizer(keyword) produced; the decoded tail
+    (window = longest keyword, in ids) is searched too.  Compared call by call with what the reference class returned
+    (tests/golden/live_reference.pt)."""
+    from videollama2_b200.mm_utils import KeywordsStoppingCriteria
+    tok = _DecodingToyTokenizer()
+    prompt = torch.zeros(1, 2, dtype=torch.long)
+    ours = KeywordsStoppingCriteria(["hello"], tok, prompt)
+    got = [ours(c, None) for c in keyword_cases(tok)]
     assert got[0] is True and got[2] is False and got[6] is False and got[7] is True
     assert got[1] is True          # id tail differs from tokenizer("hello"), the decoded window contains it
-    from oracle import ref_loader
-    if ref_loader.available():
-        import importlib
-        ref_loader.load()
-        ref_cls = importlib.import_module("videollama2.mm_utils").KeywordsStoppingCriteria
-        ref = ref_cls(["hello"], tok, prompt)
-        assert got == [bool(ref(c, None)) for c in cases]
+    assert got == _live_gold()["keywords_decoded"]

@@ -58,8 +58,8 @@ def test_gemm_every_tile_width(cuda, bn):
 @pytest.mark.parametrize("bn", [128, 160, 192, 224, 256])
 @pytest.mark.parametrize("M,N,K", [(1100, 2072, 328), (100, 512, 64), (130, 264, 136), (256, 256, 64), (9232, 1024, 192)])
 def test_gemm_cta_pair_kernel(cuda, bn, M, N, K):
-    """cta_group::2 kernel (two CTAs per 256 x BN tile): every width; persistent multi-tile loops; M tails where the
-    peer CTA's half is partly or entirely out of bounds; N/K tails."""
+    """Two-CTA cluster kernel (two CTAs per 256 x BN tile, B tile multicast to both): every width; persistent multi-tile
+    loops; M tails where the peer CTA's half is partly or entirely out of bounds; N/K tails."""
     from videollama2_b200 import ops
     a = rnd((M, K), cuda, seed=60)
     w = rnd((N, K), cuda, 0.06, seed=61)
@@ -104,13 +104,13 @@ def test_gemm_epilogue(cuda, act, with_res):
 
 
 @pytest.mark.parametrize("M,N,K,bn,kind", [
-    (1776, 4096, 4096, 0, "res_sumsq"),      # decoder o_proj: 112 pair tiles on 74 pairs -> 38 tiles split in 2
-    (1776, 6144, 4096, 0, "bias"),           # decoder QKV: 168 pair tiles -> 20 tiles split in 3
+    (1776, 4096, 4096, 0, "res_sumsq"),      # decoder o_proj: 112 pair tiles on 66 pairs -> 46 tiles split
+    (1776, 6144, 4096, 0, "bias"),           # decoder QKV: 196 pair tiles on 66 pairs -> 64 tiles split
     (1776, 4096, 1024, 1256, "plain"),       # short K: 16 k-blocks -> 2 slices of 8
-    (1200, 4096, 2048, 256, "res_sumsq"),    # single-CTA tiles: 160 tiles on 148 SMs -> 12 tiles split in 4
+    (1200, 4096, 2048, 256, "res_sumsq"),    # single-CTA tiles: 160 tiles on 132 SMs -> 28 tiles split in 4
     (1776, 28672, 512, 0, "swiglu"),         # SwiGLU epilogue on an owner tile
     (300, 520, 256, 0, "bias"),              # one round, short K: nothing to split
-    (1154, 1024, 4096, 0, "res_sumsq"),      # ViT fc2 of a 2-frame shard: 20 pair tiles for 74 pairs -> 3 slices each
+    (1154, 1024, 4096, 0, "res_sumsq"),      # ViT fc2 of a 2-frame shard: one partial round of pair tiles
     (1776, 4096, 14336, 0, "res_sumsq"),     # decoder down_proj
 ])
 @pytest.mark.parametrize("slices", [2, 3, 4])
@@ -550,7 +550,7 @@ def test_gemm_rope_epilogue(cuda, S, Hq, Hkv, D, pos0, bn, with_bias):
 
 @pytest.mark.parametrize("F,H,P,C", [(2, 336, 14, 1024), (3, 56, 14, 128), (1, 112, 14, 256), (16, 336, 14, 1024)])
 def test_patch_embed_fused_clip(cuda, F, H, P, C):
-    """vl2_patch_embed (patch gather -> tcgen05 conv -> + position -> class row -> pre-LayerNorm in ONE kernel) against
+    """vl2_patch_embed (patch gather -> wgmma conv -> + position -> class row -> pre-LayerNorm in ONE kernel) against
     conv2d + cat(cls) + position + layer_norm in fp32, and against the three-kernel explicit path it replaces."""
     from videollama2_b200 import ops
     px = rnd((F, 3, H, H), cuda, seed=16)
@@ -593,16 +593,14 @@ def test_patch_embed_fused_siglip(cuda, F, H, P, C):
     assert tok.shape == ref.shape and relerr(tok, ref) < 4e-3
 
 
-@pytest.mark.parametrize("bn", [0, 64, 160, 224, 1128, 1224, 1256, 2416])
+@pytest.mark.parametrize("bn", [64, 96, 128, 160, 192, 224, 256, 1128, 1160, 1192, 1224, 1256])
 @pytest.mark.parametrize("kind", ["bias_act_res", "rms_stats", "swiglu", "plain_tail", "inplace_strided"])
-def test_gemm_lean_and_general_epilogues_agree(cuda, bn, kind):
-    """The lean epilogue (32-column units, TMA stores, residual blocks by TMA load one unit ahead) against the general one
-    (smem transpose + st.global) on the same launch: same arithmetic, so the outputs must agree to the last bf16 bit up to
-    FMA contraction (<= 1 ulp on a handful of elements), and both against the fp32 restatement.  M / N tails, several
-    tiles per CTA (the cross-tile residual prefetch), every tile family."""
+def test_gemm_epilogue_kinds_agree_across_tiles(cuda, bn, kind):
+    """Every epilogue family on a forced tile (single-CTA widths and two-CTA pair tiles) against the tile the cost model
+    picks on the same launch: same arithmetic per output element, so the outputs agree up to FMA contraction and the
+    k-block order of the accumulation, and both against the fp32 restatement.  M / N tails, several tiles per CTA, an
+    output that aliases the residual inside a wider buffer (nothing outside the slice may be written)."""
     from videollama2_b200 import ops
-    if kind == "swiglu" and bn in (160, 224, 1224, 2416):
-        pytest.skip("SwiGLU with a tile width that is not a multiple of 64 always takes the general epilogue (no wide SwiGLU tile)")
     M, N, K = (9232, 1048, 192) if kind == "plain_tail" else (2100, 2080, 328)
     a = rnd((M, K), cuda, seed=70)
     w = rnd((N, K), cuda, 0.06, seed=71)
@@ -623,10 +621,8 @@ def test_gemm_lean_and_general_epilogues_agree(cuda, bn, kind):
         ref = torch.nn.functional.silu(ref[:, 0::2]) * ref[:, 1::2]
         kw = dict(act=ops.ACT_SWIGLU)
     outs = []
-    for i, general in enumerate((False, True)):
+    for i, tile in enumerate((bn, 0)):
         k2 = dict(kw)
-        if general and bn == 2416:
-            bn = 1224          # the wide (224 + 192, two accumulators) tile exists for the lean epilogue only
         if stats is not None:
             k2.update(sumsq_out=stats[i][0], rowsum_out=stats[i][1])
         if kind == "inplace_strided":
@@ -635,11 +631,11 @@ def test_gemm_lean_and_general_epilogues_agree(cuda, bn, kind):
             view = buf[:, 32:32 + N]
             if i == 0:
                 ref = ref + view.float()
-            outs.append(ops.gemm(a, w, residual=view, out=view, bn=bn, general_epilogue=general).clone())
+            outs.append(ops.gemm(a, w, residual=view, out=view, bn=tile).clone())
             assert torch.equal(buf[:, :32], rnd((M, N + 64), cuda, seed=74)[:, :32]), "store outside the output slice"
             assert torch.equal(buf[:, 32 + N:], rnd((M, N + 64), cuda, seed=74)[:, 32 + N:]), "store outside the output slice"
         else:
-            outs.append(ops.gemm(a, w, bn=bn, general_epilogue=general, **k2))
+            outs.append(ops.gemm(a, w, bn=tile, **k2))
     assert relerr(outs[0], ref) < 6e-3 and relerr(outs[1], ref) < 6e-3, (kind, bn)
     diff = (outs[0].float() - outs[1].float()).abs()
     assert (diff > 0).float().mean().item() < 1e-3 and relerr(outs[0], outs[1]) < 1e-4, (kind, bn, diff.max().item())
@@ -648,49 +644,3 @@ def test_gemm_lean_and_general_epilogues_agree(cuda, bn, kind):
         for (sq, sm) in stats:
             assert torch.allclose(sq.sum(1), (o ** 2).sum(1), rtol=2e-3, atol=1e-2)
             assert torch.allclose(sm.sum(1), o.sum(1), rtol=2e-3, atol=0.5)
-
-
-@pytest.mark.parametrize("M,N,K", [(1776, 4096, 512), (600, 1000, 192), (9232, 4096, 128), (100, 424, 64), (257, 8, 72)])
-def test_gemm_wide_two_accumulator_tile(cuda, M, N, K):
-    """The 256 x 416 cta_group::2 tile (two TMEM accumulators of 224 and 192 columns sharing every A k-block, one accumulator
-    stage): forced through the test hook, against fp32 and against the narrow pair tile.  Several rounds per CTA
-    (9232 x 4096: 370 tiles on 74 pairs) exercise the un-overlapped accumulator hand-over; N tails end inside the first
-    or the second accumulator, or (N = 8) leave the second one entirely out of bounds."""
-    from videollama2_b200 import ops
-    a = rnd((M, K), cuda, seed=80)
-    w = rnd((N, K), cuda, 0.06, seed=81)
-    bias = torch.randn(N, device=cuda)
-    res = rnd((M, N), cuda, seed=82)
-    ref = a.float() @ w.float().t() + bias + res.float()
-    stats = N % 32 == 0
-    outs = []
-    for bn in (2416, 1224):
-        kw = {}
-        if stats:
-            kw = dict(sumsq_out=torch.empty((M, N // 32), device=cuda), rowsum_out=torch.empty((M, N // 32), device=cuda))
-        out = ops.gemm(a, w, bias=bias, residual=res, bn=bn, **kw)
-        assert relerr(out, ref) < 6e-3, (bn, M, N, K)
-        if stats:
-            o = out.float()
-            assert torch.allclose(kw["sumsq_out"].sum(1), (o ** 2).sum(1), rtol=2e-3, atol=1e-2)
-            assert torch.allclose(kw["rowsum_out"].sum(1), o.sum(1), rtol=2e-3, atol=0.5)
-        outs.append(out)
-    assert relerr(outs[0], outs[1]) < 1e-4
-    out2 = ops.gemm(a, w, bias=bias, residual=res, bn=2416)
-    assert torch.equal(out2, outs[0]), "the wide tile must be bit-reproducible"
-
-
-def test_gemm_wide_tile_is_chosen_for_single_round_launches(cuda):
-    """The decoder's o_proj / down_proj at S = 1776 (7 x 10 wide tiles = one round of the 74 CTA pairs) go to the wide tile
-    by the cost model; the result equals the forced narrow tile's up to accumulation order."""
-    import ctypes
-    from videollama2_b200 import _lib, ops
-    out6 = (ctypes.c_int32 * 6)()
-    assert _lib.load().vl2_gemm_plan(1776, 4096, 4096, 0, out6) == 0
-    if out6[5] != 148:
-        pytest.skip("plan pinned for 148 SMs")
-    assert (out6[0], out6[1], out6[2], out6[4]) == (416, 1, 70, 1)
-    a = rnd((1776, 4096), cuda, seed=83)
-    w = rnd((4096, 4096), cuda, 0.02, seed=84)
-    res = rnd((1776, 4096), cuda, seed=85)
-    assert relerr(ops.gemm(a, w, residual=res), ops.gemm(a, w, residual=res, bn=1224)) < 1e-4

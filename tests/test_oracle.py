@@ -44,24 +44,18 @@ def test_oracle_bf16_matches_reference_bf16(name):
 
 
 def test_oracle_vs_live_reference():
-    from oracle import ref_loader, synth, torch_ref
-    if not ref_loader.available():
-        pytest.skip("/root/reference not present (GPU box): goldens cover this")
+    """The oracle against the reference model's own fp32 outputs (tests/golden/live_reference.pt, oracle/make_golden_live.py)."""
+    from oracle import synth, torch_ref
     cfg = synth.CONFIGS["tiny"]
     sd = synth.state_dict(cfg)
     px, ids = synth.inputs(cfg)
-    m = ref_loader.build_reference_model(cfg, torch.float32, sd)
-    with torch.no_grad():
-        res = m(input_ids=ids, attention_mask=torch.ones_like(ids), images=[(px.float(), "video")])
-        stc_in = torch.randn(2, 4, 16, cfg.vision.hidden)
-        stc_ref = m.get_model().mm_projector(stc_in)
+    gold = torch.load(os.path.join(GOLD, "live_reference.pt"))["tiny"]
     mine = torch_ref.full_forward(sd, cfg, px, ids, torch.float32)
-    assert rel(mine["logits"], res.logits[0]) < 1e-5
-    assert rel(torch_ref.stc_forward(sd, stc_in, 1, 4, torch.float32), stc_ref) < 1e-5      # batch of 2 videos
+    assert rel(mine["logits"], gold["logits"]) < 1e-5
+    assert rel(torch_ref.stc_forward(sd, gold["stc_in"], 1, 4, torch.float32), gold["stc"]) < 1e-5      # batch of 2 videos
     # state-dict contract: names and shapes of the synthetic weights are exactly the reference model's
-    ref_sd = m.state_dict()
     mine_names = {n: tuple(s) for n, s, _ in synth.model_specs(cfg)}
-    assert {k: tuple(v.shape) for k, v in ref_sd.items()} == mine_names
+    assert gold["state_dict_shapes"] == mine_names
 
 
 def test_flop_model_matches_baseline_md():

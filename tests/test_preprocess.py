@@ -9,11 +9,14 @@ import pytest
 import torch
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "preprocess.pt")
+GOLD_HD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "preprocess_hd.pt")   # the 640 x 360 case
 
 
 @pytest.fixture(scope="module")
 def gold():
-    return torch.load(GOLD)
+    g = torch.load(GOLD)
+    g["cases"].update(torch.load(GOLD_HD)["cases"])
+    return g
 
 
 def test_oracle_resample_matches_pillow_live():

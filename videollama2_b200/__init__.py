@@ -1,7 +1,7 @@
-"""videollama2_b200 — B200 (sm_100a) engine for VideoLLaMA2's video->text path.
+"""videollama2_b200 — H100 (sm_90a) engine for VideoLLaMA2's video->text path.
 
 Host code is Python/PyTorch (memory, streams, torch.distributed); all arithmetic runs in libvl2.so
-(hand-written CUDA: tcgen05/TMEM/TMA GEMM + attention, fused row kernels) through the C-ABI in include/vl2.h.
+(hand-written CUDA: wgmma/TMA GEMM + attention, fused row kernels) through the C-ABI in include/vl2.h.
 
 `model_init` / `mm_infer` mirror the reference's two user-facing calls (videollama2/__init__.py:14-36, 39-114): the
 callers on either side of the accelerated path.  Everything heavy is imported lazily so that `import videollama2_b200`
@@ -76,7 +76,7 @@ def build_messages(instruct, modal: str, model_type: str):
 
 
 def mm_infer(image_or_video, instruct, model, tokenizer, modal="video", **kwargs):
-    """Inference API of the reference (videollama2/__init__.py:39-114) on the B200 engine: prompt construction and
+    """Inference API of the reference (videollama2/__init__.py:39-114) on the H100 engine: prompt construction and
     stopping criteria on the host (exact), vision + prefill + graph-replayed decode on the device.  Greedy only."""
     import torch
     from .mm_utils import KeywordsStoppingCriteria, tokenizer_multimodal_token

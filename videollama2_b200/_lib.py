@@ -1,5 +1,5 @@
 """ctypes binding of libvl2.so (include/vl2.h).  There is NO fallback: if the library is missing the import of any
-compute entry point raises, and on a box without an sm_100 GPU every compute call returns VL2_E_CUDA."""
+compute entry point raises, and on a box without an sm_90 GPU every compute call returns VL2_E_CUDA."""
 from __future__ import annotations
 
 import ctypes as C
@@ -12,7 +12,7 @@ LIB_PATH_F16 = os.environ.get("VL2_LIBVL2_F16") or os.path.join(_HERE, "libvl2_f
 # Every symbol include/vl2.h declares (tests/test_abi.py checks the header against this list and the .so).
 SYMBOLS = [
     "vl2_version", "vl2_storage_dtype", "vl2_last_error", "vl2_launch_count",
-    "vl2_gemm_bf16", "vl2_gemm_skinny", "vl2_attention", "vl2_attention_decode", "vl2_debug_attn_trace", "vl2_debug_attn_timeline", "vl2_debug_gemm_trace", "vl2_gemm_plan",
+    "vl2_gemm_bf16", "vl2_gemm_skinny", "vl2_attention", "vl2_attention_decode", "vl2_debug_attn_trace", "vl2_debug_gemm_trace", "vl2_gemm_plan",
     "vl2_decode_rope_append", "vl2_attention_decode_dyn", "vl2_gemv_bf16", "vl2_attention_decode_workspace", "vl2_set_pdl", "vl2_l2_prefetch", "vl2_preprocess_frames", "vl2_preprocess_workspace",
     "vl2_layernorm", "vl2_rmsnorm", "vl2_row_sumsq", "vl2_row_stats",
     "vl2_patch_im2col", "vl2_clip_embed_finish",
@@ -99,7 +99,7 @@ def load(dtype=None) -> C.CDLL:
     path = LIB_PATH if var == "bf16" else LIB_PATH_F16
     if not os.path.exists(path):
         raise Vl2Error(
-            f"{path} is missing: build it with `python -m videollama2_b200.build` (nvcc, sm_100a). "
+            f"{path} is missing: build it with `python -m videollama2_b200.build` (nvcc, sm_90a). "
             "videollama2_b200 has no CPU or PyTorch fallback.")
     lib = C.CDLL(path)
     vp, i32, i64, f32 = C.c_void_p, C.c_int, C.c_int64, C.c_float
@@ -110,7 +110,6 @@ def load(dtype=None) -> C.CDLL:
         "vl2_gemm_bf16": [C.POINTER(GemmArgs), vp],
         "vl2_gemm_skinny": [vp, i32, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp],
         "vl2_debug_attn_trace": [vp],
-        "vl2_debug_attn_timeline": [vp],
         "vl2_debug_gemm_trace": [vp],
         "vl2_gemm_plan": [i32, i32, i32, i32, vp],
         "vl2_decode_rope_append": [vp, vp, i64, vp, i32, i32, i32, vp, i32, vp],

@@ -1,7 +1,7 @@
-"""Build libvl2.so (the sm_100a kernel library + C-ABI) in-tree with nvcc.
+"""Build libvl2.so (the sm_90a kernel library + C-ABI) in-tree with nvcc.
 
-`python -m videollama2_b200.build` or `__graft_entry__.build()`.  nvcc cross-compiles without a GPU.  The .so is
-git-ignored but travels to the GPU box with the gpurun snapshot.
+`python -m videollama2_b200.build` or `__graft_entry__.build()`.  nvcc cross-compiles without a GPU.  The libraries and
+object files are build products (git-ignored).
 """
 from __future__ import annotations
 
@@ -18,7 +18,7 @@ OUT = os.path.join(HERE, "libvl2.so")
 OBJ_DIR = os.path.join(HERE, "build")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -91,8 +91,8 @@ def build(force: bool = False, verbose: bool = False) -> str:
                 raise RuntimeError(f"nvcc failed on {src}")
     for name, out, obj_dir, defs, stamp in todo:
         objs = [os.path.join(obj_dir, os.path.basename(s)[:-3] + ".o") for s in srcs]
-        tmp = out + ".tmp"   # link next to the target, then rename: a reader (or a gpurun snapshot) never sees a partial library
-        link = [nvcc, "-shared", "-o", tmp, *objs, "-gencode", "arch=compute_100a,code=sm_100a"]
+        tmp = out + ".tmp"   # link next to the target, then rename: a reader never sees a partial library
+        link = [nvcc, "-shared", "-o", tmp, *objs, "-gencode", "arch=compute_90a,code=sm_90a"]
         r = subprocess.run(link, capture_output=True, text=True)
         if r.returncode != 0:
             sys.stderr.write(r.stdout + r.stderr)

@@ -1,0 +1,719 @@
+// Persistent warp-specialised bf16 GEMM for sm_90a:  C[M,Nout] = epi(A[M,K] * W[N,K]^T).
+//
+//   warpgroup 0   TMA producer (one thread): cp.async.bulk.tensor A/B tiles -> 128B-swizzled smem ring
+//   warpgroups 1, 2  consumers: wgmma.mma_async m64 x BN x k16 from the ring (rows 0..63 / 64..127 of the 128-row tile),
+//                 fp32 accumulators in registers, then the epilogue straight from the accumulator fragments:
+//                 row_scale / folded RMSNorm or LayerNorm / bias / activation / SwiGLU / RoPE / residual / statistics
+//                 -> global (optionally also to peer buffers or an NVSwitch multicast address)
+//
+// Tiles are 128 x BN, BN in {64,...,256} step 32 chosen per launch by a wave / operand-traffic cost model (choose_tile);
+// BLOCK_K = 64 bf16 = one 128-byte swizzle atom; the grid is persistent (<= #SMs CTAs, static round-robin over tiles,
+// M fastest so that a wave shares W tiles through L2).  M/N/K tails: TMA zero-fills out-of-bounds reads, stores are
+// predicated.
+#include <stdlib.h>
+
+#include "host_common.h"
+#include "ptx.cuh"
+
+namespace vl2 {
+
+static constexpr int BM = 128;
+static constexpr int BK = 64;
+static constexpr int kConsumerThreads = 256;              // two consumer warpgroups
+static constexpr int kGemmThreads = 128 + kConsumerThreads;
+static constexpr int kConvLine = 16;                      // Conv3d front end: output lines and columns per time step are padded to 16
+
+// PAIR = true: the two CTAs of a cluster compute a 256 x BN tile (128 rows each) and share its B tile: each CTA loads
+// HALF of the B rows and the TMA unit multicasts them into both CTAs' shared memory, so a k-block costs
+// 16 KB + BN*64 B of L2 traffic per CTA instead of 16 KB + BN*128 B.  A ring slot is free once the consumers of BOTH
+// CTAs have read it (the peer's multicast writes into it), so every consumer warp releases it in both CTAs.
+template <int BN, bool PAIR>
+struct GemmCfg {
+  static_assert(BN % 32 == 0 && BN >= 64 && BN <= 256, "BN must be a multiple of 32 in [64,256]");
+  static_assert(!PAIR || BN >= 128, "a pair tile is at least 128 columns wide");
+  static constexpr int kStageBytesA = BM * BK * 2;
+  static constexpr int kStageBytesB = BN * BK * 2;
+  static constexpr int kHalfBytesB = BN / 2 * BK * 2;     // pair: the half of B one CTA loads (1024-byte multiple)
+  static constexpr int kStageBytes = kStageBytesA + kStageBytesB;
+  static constexpr int kExtraBytes = 1024;               // barriers
+  static constexpr int kMaxStages = (227 * 1024 - kExtraBytes) / kStageBytes;
+  static constexpr int kStages = kMaxStages > 8 ? 8 : kMaxStages;
+  static constexpr int kSmemBytes = kStages * kStageBytes + kExtraBytes;
+  static constexpr int kAcc = BN / 2;                     // fp32 accumulators per consumer thread
+  static constexpr int kEmptyArrivals = (PAIR ? 2 : 1) * (kConsumerThreads / 32);
+  static_assert(!PAIR || kHalfBytesB % 1024 == 0, "the peer's half of B must start on a swizzle-atom boundary");
+};
+
+struct GemmParams {
+  void* C;
+  const float* bias;
+  const void* residual;
+  const float* row_scale;
+  int64_t ldc, ldr;
+  int M, N, K;
+  int act;
+  int out_f32;
+  int num_m_tiles, num_n_tiles;
+  // epilogue-fused all-gather: peers' copies of C (NVLink P2P stores) or one NVSwitch multicast address
+  __nv_bfloat16* bcast[8];
+  __nv_bfloat16* mc;
+  int n_bcast;
+  // folded RMSNorm / LayerNorm (see vl2.h)
+  const float* rms_sumsq_in;
+  const float* ln_sum_in;
+  const float* ln_colsum;
+  float* rowsum_out;
+  float* sumsq_out;
+  int rms_nparts;
+  float rms_inv_dim, rms_eps;
+  // split-K of the last, partial round (see launch_gemm): items >= split_first are K-slices of the remaining tiles
+  int split_first, split_s, num_items;
+  float* ws_partial;      // [tiles past split_first][split_s - 1][tile rows][BN] fp32 partial accumulators
+  unsigned* ws_flags;     // [tiles past split_first][2] arrival counters (self-resetting)
+  // implicit-GEMM Conv3d(k = s = 2) front end (see vl2.h: conv_C > 0).  A rows are the output positions in a padded
+  // enumeration (to, ho16, wo16): 16 x 16 rows per output time step, so that one 128-row tile is 8 whole output lines of
+  // one time step and a k-block (one tap x 64 channels) of the tile is ONE 5-D TMA box over x viewed as
+  // [T, H/2, 2, W/2, 2C] (the stride-2 walks along H and W become unit walks over the coarse indices at a fixed parity);
+  // the spatial zero padding and the padded rows are TMA out-of-bounds fill.
+  int conv_C, conv_pad, conv_Ho, conv_Wo, conv_To;
+  // RoPE in the QKV epilogue (see vl2.h): adjacent output columns (2i, 2i+1) of a head are a rotation pair
+  const uint32_t* rope_tab;
+  int rope_cols, rope_D, rope_pos0;
+  int trace;   // debug: CTA 0 records clock64() at item boundaries of its first consumer thread (vl2_debug_gemm_trace)
+};
+
+// [0] items traced; per item t (<= 7), at 8*t + 4: consumer starts the item, 8*t + 5: accumulator complete,
+// 8*t + 6: its part of the tile is stored.
+__device__ long long g_gemm_trace[128];
+
+// one 4-byte store replicated by the NVSwitch to every GPU of the multicast group
+__device__ __forceinline__ void multimem_st32(void* mc_addr, uint32_t v) {
+  asm volatile("multimem.st.relaxed.sys.global.f32 [%0], %1;" ::"l"(mc_addr), "f"(__uint_as_float(v)) : "memory");
+}
+
+__device__ __forceinline__ float fast_sigmoid_mul(float x, float k_log2e) {
+  // x * sigmoid(k x) = x / (1 + 2^(-k*log2e*x)); approximate reciprocal on the MUFU pipe
+  return __fdividef(x, 1.f + fast_exp2(-k_log2e * x));
+}
+__device__ __forceinline__ float gelu_tanh(float x) {
+  // 0.5 x (1 + tanh(u)) = x * sigmoid(2u), u = sqrt(2/pi) (x + 0.044715 x^3)      (HF "gelu_pytorch_tanh", SigLIP MLP)
+  const float u2 = x * fmaf(0.0356774081f * x, x, 0.7978845608f) * 2.885390082f;   // 2 u log2(e)
+  return __fdividef(x, 1.f + fast_exp2(-u2));
+}
+__device__ __forceinline__ float act_apply(float x, int act) {
+  switch (act) {
+    case VL2_ACT_QUICK_GELU: return fast_sigmoid_mul(x, 1.702f * 1.4426950408889634f);
+    case VL2_ACT_SILU: return fast_sigmoid_mul(x, 1.4426950408889634f);
+    case VL2_ACT_GELU_ERF: return 0.5f * x * (1.f + erff(x * 0.70710678118654752f));
+    case VL2_ACT_GELU_TANH: return gelu_tanh(x);
+    default: return x;
+  }
+}
+
+// One unit of the persistent loop: a whole output tile (part = -1), or - for the tiles of the last, partial round - one
+// K-slice of a tile: part 0 owns the tile (adds the other slices' partials and runs the epilogue), parts > 0 dump their
+// fp32 accumulators to the workspace.  Every role (producer, consumers) decodes the same sequence.
+constexpr size_t kSplitFlagBytes = 65536;  // arrival counters at the head of the split-K workspace, one 128-byte line each
+constexpr int kSplitFlagStride = 32;       // (zero at first use, self-resetting)
+constexpr double kSplitOverheadCycles = 16000.0;   // dump + fence + flag + owner's partial reads
+struct WorkItem { int tile, kb0, kb1, part; };
+__device__ __forceinline__ WorkItem decode_item(int item, const GemmParams& p, int nkb) {
+  WorkItem w;
+  if (item < p.split_first) {
+    w.tile = item; w.kb0 = 0; w.kb1 = nkb; w.part = -1;
+  } else {
+    const int j = item - p.split_first;
+    w.tile = p.split_first + j / p.split_s;
+    w.part = j % p.split_s;
+    w.kb0 = (int)((long long)w.part * nkb / p.split_s);
+    w.kb1 = (int)((long long)(w.part + 1) * nkb / p.split_s);
+  }
+  return w;
+}
+__device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned* p) {
+  unsigned v;
+  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory"); }
+
+// sum the producer's per-32-column partials of one row in a fixed order (deterministic: no atomics anywhere)
+__device__ __forceinline__ float sum_parts(const float* pp, int nparts) {
+  const int nvec = (nparts % 4 == 0) ? nparts : 0;   // rows are 16-byte aligned only then
+  float q = 0.f;
+  int i = 0;
+  for (; i + 4 <= nvec; i += 4) {
+    const float4 t4 = *reinterpret_cast<const float4*>(pp + i);
+    q += (t4.x + t4.y) + (t4.z + t4.w);
+  }
+  for (; i < nparts; ++i) q += pp[i];
+  return q;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Epilogue of one consumer thread.  wgmma accumulator layout (m64 x BN, warp w of the warpgroup, lane = 4 g + t):
+//   acc[4 j + 0, 1] = rows 16 w + g,     columns 8 j + 2 t, 8 j + 2 t + 1
+//   acc[4 j + 2, 3] = rows 16 w + g + 8, the same columns
+// so a thread holds two rows and, per 8-column group, an adjacent column pair: exactly a SwiGLU (gate, up) pair and a
+// RoPE rotation pair.  The four threads of a quad (same g) together hold a row's 8 columns of every group; the
+// per-32-column statistics are reduced over the quad.
+// ---------------------------------------------------------------------------------------------------------------------
+template <int BN>
+__device__ __forceinline__ void gemm_epilogue(float (&acc)[BN / 2], const GemmParams& p, int m0, int n0, int rloc) {
+  const int lane = threadIdx.x & 31, t = lane & 3;
+  const bool swiglu = p.act == VL2_ACT_SWIGLU;
+  const bool ln = p.ln_sum_in != nullptr;
+  int rows[2];
+  float rs[2], mu[2];
+  bool ok[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = m0 + rloc + 8 * h;
+    ok[h] = row < p.M;
+    rs[h] = (p.row_scale != nullptr && ok[h]) ? p.row_scale[row] : 1.f;
+    mu[h] = 0.f;
+    if (p.rms_sumsq_in != nullptr && ok[h]) {
+      float q = sum_parts(p.rms_sumsq_in + (int64_t)row * p.rms_nparts, p.rms_nparts) * p.rms_inv_dim;   // E[x^2]
+      if (ln) {
+        mu[h] = sum_parts(p.ln_sum_in + (int64_t)row * p.rms_nparts, p.rms_nparts) * p.rms_inv_dim;
+        q = fmaxf(q - mu[h] * mu[h], 0.f);                                                          // variance
+      }
+      rs[h] *= rsqrtf(q + p.rms_eps);
+    }
+    int gr = row;
+    if (p.conv_C > 0) {   // padded (to, ho16, wo16) row -> real output row, or nothing for the padding positions
+      const int wo = gr % kConvLine, ho = (gr / kConvLine) % kConvLine, to = gr / (kConvLine * kConvLine);
+      gr = (wo < p.conv_Wo && ho < p.conv_Ho && to < p.conv_To) ? (to * p.conv_Ho + ho) * p.conv_Wo + wo : p.M;
+      ok[h] = gr < p.M;
+    }
+    rows[h] = gr;
+  }
+  const __nv_bfloat16* res = reinterpret_cast<const __nv_bfloat16*>(p.residual);
+  __nv_bfloat16* cb = reinterpret_cast<__nv_bfloat16*>(p.C);
+#pragma unroll
+  for (int s = 0; s < BN / 32; ++s) {      // 32-column slots
+    if (n0 + 32 * s >= p.N) break;         // uniform over the warpgroup
+    float ssq[2] = {0.f, 0.f}, ssum[2] = {0.f, 0.f};
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj) {
+      const int j = 4 * s + jj;
+      const int c = n0 + 8 * j + 2 * t;    // this thread's column pair
+      const bool col_ok = n0 + 8 * j < p.N;   // N % 8 == 0: the whole 8-column group is in or out
+      float2 bq = make_float2(0.f, 0.f), cs = make_float2(0.f, 0.f);
+      if (col_ok && p.bias != nullptr) bq = __ldg(reinterpret_cast<const float2*>(p.bias + c));
+      if (col_ok && ln) cs = __ldg(reinterpret_cast<const float2*>(p.ln_colsum + c));
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
+        if (ln) { x0 = fmaf(-mu[h], cs.x, x0); x1 = fmaf(-mu[h], cs.y, x1); }
+        x0 = x0 * rs[h] + bq.x;
+        x1 = x1 * rs[h] + bq.y;
+        const bool st_ok = col_ok && ok[h];
+        if (swiglu) {
+          // (gate, up) -> one output at column c / 2; the even lane of a lane pair stores both lanes' outputs
+          const float o = fast_sigmoid_mul(x0, 1.4426950408889634f) * x1;
+          const float o_next = __shfl_down_sync(0xffffffffu, o, 1);
+          if (st_ok && (t & 1) == 0) {
+            *reinterpret_cast<uint32_t*>(cb + (int64_t)rows[h] * p.ldc + (c >> 1)) = pack_bf16(o, o_next);
+          }
+          continue;
+        }
+        x0 = act_apply(x0, p.act);
+        x1 = act_apply(x1, p.act);
+        if (p.rope_tab != nullptr && c < p.rope_cols && st_ok) {
+          const uint32_t e = __ldg(p.rope_tab + (int64_t)(p.rope_pos0 + rows[h]) * (p.rope_D >> 1) + ((c % p.rope_D) >> 1));
+          const float co = bf16_lo(e), sn = bf16_hi(e);
+          const float a = x0, b = x1;
+          x0 = a * co - b * sn;
+          x1 = b * co + a * sn;
+        }
+        if (res != nullptr && st_ok) {
+          const uint32_t r = *reinterpret_cast<const uint32_t*>(res + (int64_t)rows[h] * p.ldr + c);
+          x0 += bf16_lo(r);
+          x1 += bf16_hi(r);
+        }
+        if (p.out_f32) {
+          if (st_ok) *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.C) + (int64_t)rows[h] * p.ldc + c) = make_float2(x0, x1);
+          continue;
+        }
+        const uint32_t pk = pack_bf16(x0, x1);
+        if (st_ok) {
+          const int64_t off = (int64_t)rows[h] * p.ldc + c;
+          *reinterpret_cast<uint32_t*>(cb + off) = pk;
+          if (p.mc != nullptr) {
+            multimem_st32(p.mc + off, pk);
+          } else {
+            for (int pi = 0; pi < p.n_bcast; ++pi) *reinterpret_cast<uint32_t*>(p.bcast[pi] + off) = pk;
+          }
+        }
+        const float a0 = bf16_lo(pk), a1 = bf16_hi(pk);   // statistics of what the consumer will read
+        ssq[h] += a0 * a0 + a1 * a1;
+        ssum[h] += a0 + a1;
+      }
+    }
+    if (p.sumsq_out != nullptr) {   // one slot per 32 output columns (N % 32 == 0), reduced over the quad
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float q = ssq[h], sm = ssum[h];
+        q += __shfl_xor_sync(0xffffffffu, q, 1);
+        q += __shfl_xor_sync(0xffffffffu, q, 2);
+        sm += __shfl_xor_sync(0xffffffffu, sm, 1);
+        sm += __shfl_xor_sync(0xffffffffu, sm, 2);
+        if (t == 0 && ok[h]) {
+          const int64_t slot = (int64_t)rows[h] * (p.N >> 5) + ((n0 >> 5) + s);
+          p.sumsq_out[slot] = q;
+          if (p.rowsum_out != nullptr) p.rowsum_out[slot] = sm;
+        }
+      }
+    }
+  }
+}
+
+template <int BN, bool PAIR>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                       const GemmParams p) {
+  using Cfg = GemmCfg<BN, PAIR>;
+  const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
+  const int tile0 = PAIR ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;        // persistent tile loop start / stride
+  const int tile_stride = PAIR ? (int)(gridDim.x >> 1) : (int)gridDim.x;
+  constexpr int kTileM = PAIR ? 2 * BM : BM;
+  // SWIZZLE_128B operands need 1024-byte aligned stage bases: the kernel has no static smem, so the dynamic window
+  // starts at offset 0 of the CTA's shared memory (checked below; a misaligned base traps instead of corrupting).
+  extern __shared__ __align__(1024) uint8_t smem[];
+  if ((smem_u32(smem) & 1023u) != 0) { asm volatile("trap;"); }
+  uint8_t* smem_a = smem;
+  uint8_t* smem_b = smem + Cfg::kStages * Cfg::kStageBytesA;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
+  uint64_t* full_bar = bars;                        // [kStages]  TMA -> consumers
+  uint64_t* empty_bar = bars + Cfg::kStages;        // [kStages]  consumers (of both CTAs of a pair) -> TMA
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int num_k_blocks = (p.K + BK - 1) / BK;
+
+  pdl_launch_dependents();   // let the next kernel's CTAs take the SMs this kernel's last wave leaves idle
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmap_a);
+    tma_prefetch_desc(&tmap_b);
+    for (int i = 0; i < Cfg::kStages; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], Cfg::kEmptyArrivals);
+    }
+    fence_barrier_init();
+  }
+  pdl_wait();                // predecessors complete + visible: nothing above touched global memory
+  if (PAIR) cluster_sync_all(); else __syncthreads();   // barrier inits visible (cluster-wide for a pair)
+
+  if (warp < 4) {
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      // ===================== TMA producer =====================
+      int stage = 0;
+      uint32_t phase = 0;
+      const bool conv = p.conv_C > 0;
+      const int slabs = conv ? p.conv_C / BK : 1;
+      for (int item = tile0; item < p.num_items; item += tile_stride) {
+        const WorkItem w = decode_item(item, p, num_k_blocks);
+        const int m0 = (w.tile % p.num_m_tiles) * kTileM + (int)rank * BM;
+        const int n0 = (w.tile / p.num_m_tiles) * BN;
+        // conv: this 128-row tile = output lines ho_base .. ho_base + 7 of time step `to`
+        const int line0 = m0 / kConvLine, to = line0 / kConvLine, ho_base = line0 % kConvLine;
+        int tap = w.kb0 / slabs, slab = w.kb0 - tap * slabs;
+        for (int kb = w.kb0; kb < w.kb1; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);   // a pair: own A + both halves of B land here
+          uint8_t* dst_a = smem_a + stage * Cfg::kStageBytesA;
+          if (conv) {
+            // implicit im2col: k-block = (tap, 64-channel slab).  Input index along each axis = 2 * out + e, e = d - pad in
+            // {-1, 0, 1}: parity e & 1, coarse index out + floor(e / 2)  (-1 = the zero-padded border -> out of bounds)
+            const int et = (tap >> 2) - p.conv_pad, eh = ((tap >> 1) & 1) - p.conv_pad, ew = (tap & 1) - p.conv_pad;
+            const int ph = eh & 1, pw = ew & 1;
+            const int c0 = pw * p.conv_C + slab * BK, wc0 = (ew - pw) / 2, hc0 = ho_base + (eh - ph) / 2, t = 2 * to + et;
+            tma_load_5d(dst_a, &tmap_a, &full_bar[stage], c0, wc0, ph, hc0, t);
+            if (++slab == slabs) { slab = 0; ++tap; }
+          } else {
+            tma_load_2d(dst_a, &tmap_a, &full_bar[stage], kb * BK, m0);
+          }
+          uint8_t* dst_b = smem_b + stage * Cfg::kStageBytesB;
+          if (PAIR) tma_load_2d_mc(dst_b + rank * Cfg::kHalfBytesB, &tmap_b, &full_bar[stage], kb * BK, n0 + (int)rank * (BN / 2), 3);
+          else tma_load_2d(dst_b, &tmap_b, &full_bar[stage], kb * BK, n0);
+          if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+  } else {
+    setmaxnreg_inc<232>();
+    // ===================== consumers: wgmma main loop + epilogue =====================
+    const int wg = (warp >> 2) - 1;              // 0 / 1: rows [64 wg, 64 wg + 64) of the CTA's 128-row block
+    const int ctid = threadIdx.x - 128;
+    const int rloc = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // first of this thread's two accumulator rows
+    const uint64_t da0 = gmma_desc_sw128(smem_u32(smem_a) + wg * 64 * 128, 16, 1024);
+    const uint64_t db0 = gmma_desc_sw128(smem_u32(smem_b), 16, 1024);
+    const bool tr = p.trace && blockIdx.x == 0 && ctid == 0;
+    int stage = 0;
+    uint32_t phase = 0;
+    int it = 0;
+    float acc[Cfg::kAcc];
+    for (int item = tile0; item < p.num_items; item += tile_stride, ++it) {
+      const WorkItem w = decode_item(item, p, num_k_blocks);
+      const int tile = w.tile;
+      if (tr && it < 7) g_gemm_trace[8 * it + 4] = clock64();
+      const int m0 = (tile % p.num_m_tiles) * kTileM + (int)rank * BM;
+      const int n0 = (tile / p.num_m_tiles) * BN;
+      int prev = -1;
+      for (int kb = w.kb0; kb < w.kb1; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        wgmma_fence();
+        const uint64_t da = da0 + (uint64_t)((stage * Cfg::kStageBytesA) >> 4);
+        const uint64_t db = db0 + (uint64_t)((stage * Cfg::kStageBytesB) >> 4);
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k) Wgmma<BN, 0>::ss(acc, da + 2 * k, db + 2 * k, (kb != w.kb0 || k != 0) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();            // the previous k-block's MMAs are complete: its ring slot can be refilled
+        if (prev >= 0 && lane == 0) {
+          if (PAIR) { mbar_arrive_cluster(&empty_bar[prev], 0); mbar_arrive_cluster(&empty_bar[prev], 1); }
+          else mbar_arrive(&empty_bar[prev]);
+        }
+        prev = stage;
+        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      wgmma_keep(acc);
+      if (lane == 0) {
+        if (PAIR) { mbar_arrive_cluster(&empty_bar[prev], 0); mbar_arrive_cluster(&empty_bar[prev], 1); }
+        else mbar_arrive(&empty_bar[prev]);
+      }
+      if (tr && it < 7) g_gemm_trace[8 * it + 5] = clock64();
+      const int slot = (tile - p.split_first) * (p.split_s - 1);   // workspace slot of a split tile's slices
+      // partials layout per CTA: [accumulator quad][consumer thread][4 floats] (every warp access is one 512-byte piece)
+      if (w.part > 0) {
+        // ---- K-slice of a split tile: dump the fp32 accumulators, then signal the owner
+        float* dst = p.ws_partial + ((size_t)slot + (w.part - 1)) * ((size_t)kTileM * BN) + (size_t)rank * (BM * BN) + ctid * 4;
+#pragma unroll
+        for (int q = 0; q < Cfg::kAcc / 4; ++q)
+          __stcg(reinterpret_cast<float4*>(dst + q * (kConsumerThreads * 4)),
+                 make_float4(acc[4 * q], acc[4 * q + 1], acc[4 * q + 2], acc[4 * q + 3]));
+        __threadfence();
+        consumer_sync();   // every thread's partials are fenced
+        if (ctid == 0) atomicAdd(p.ws_flags + ((tile - p.split_first) * 2 + (int)rank) * kSplitFlagStride, 1u);
+        continue;
+      }
+      if (w.part == 0) {
+        // owner of a split tile: the other K-slices run concurrently on other CTAs of this (last) round.  ONE thread polls
+        // (a line of its own per counter): hundreds of pollers on one L2 line starve the arriving atomics
+        unsigned* flag = p.ws_flags + ((tile - p.split_first) * 2 + (int)rank) * kSplitFlagStride;
+        if (ctid == 0) {
+          unsigned spins = 0;
+          while (ld_acquire_gpu(flag) < (unsigned)(p.split_s - 1)) {
+            if (++spins > (1u << 24)) { asm volatile("trap;"); }
+            __nanosleep(200);
+          }
+        }
+        consumer_sync();
+        const float* src = p.ws_partial + (size_t)slot * ((size_t)kTileM * BN) + (size_t)rank * (BM * BN) + ctid * 4;
+        for (int pp = 0; pp < p.split_s - 1; ++pp) {   // fixed order: deterministic
+#pragma unroll
+          for (int q = 0; q < Cfg::kAcc / 4; ++q) {
+            const float4 t4 = __ldcg(reinterpret_cast<const float4*>(src + (size_t)pp * ((size_t)kTileM * BN) + q * (kConsumerThreads * 4)));
+            acc[4 * q] += t4.x; acc[4 * q + 1] += t4.y; acc[4 * q + 2] += t4.z; acc[4 * q + 3] += t4.w;
+          }
+        }
+        consumer_sync();   // every thread has consumed the partials: re-arm the counter for the next launch
+        if (ctid == 0) *flag = 0u;
+      }
+      gemm_epilogue<BN>(acc, p, m0, n0, rloc);
+      if (tr && it < 7) { g_gemm_trace[8 * it + 6] = clock64(); g_gemm_trace[0] = it + 1; }
+    }
+  }
+  if (PAIR) cluster_sync_all();   // no CTA leaves while its peer may still multicast into it or arrive on its barriers
+}
+
+static bool splitk_enabled();
+
+// Tile choice: a launch costs waves x tile time + one epilogue; a tile costs k-blocks x kb_cycles.  A k-block of a
+// 128 x BN tile is bound by the larger of
+//   * the tensor pipe: 128 x BN x 64 MACs at ~1024 dense bf16 MACs per clock per SM (the H100 SXM data sheet's
+//     989 TFLOP/s over 132 SMs at 1.83 GHz), i.e. 8 x BN cycles, plus ~200 cycles per k-block of barrier hand-over
+//     and issue that a wider tile amortises over more columns;
+//   * operand ingest from L2: 16 KB of A + the CTA's B bytes (all BN rows, or BN / 2 for a pair) at ~64 B/clk;
+//   * the ring's latency cover: ~2000 cycles of L2/HBM latency over the ring's stages.
+struct TileChoice { int bn; bool pair; };
+static constexpr double kIngestBytesPerClk = 64.0;
+
+static double kb_cycles(int bn, bool pair) {
+  const double stage_bytes = 16384.0 + bn * 128.0;
+  int stages = (int)((227 * 1024 - 1024) / stage_bytes);
+  if (stages > 8) stages = 8;
+  const double mma = 128.0 * bn * 64.0 / 1024.0 + 200.0;
+  const double ingest = (16384.0 + (pair ? bn / 2 : bn) * 128.0) / kIngestBytesPerClk;
+  const double lat = 2000.0 / stages;
+  double c = mma > ingest ? mma : ingest;
+  return c > lat ? c : lat;
+}
+
+
+template <int BN, bool PAIR>
+static int launch_gemm(const vl2_gemm_args* a, cudaStream_t stream) {
+  using Cfg = GemmCfg<BN, PAIR>;
+  CUtensorMap ta, tb;
+  const bool conv = a->conv_C > 0;
+  int conv_To = 0, conv_Ho = 0, conv_Wo = 0;
+  if (conv) {
+    // x [T,H,W,C] viewed as [T, H/2, 2, W/2, 2C]: a tap's stride-2 walks along H and W are unit walks over the coarse
+    // indices at fixed parities (the W parity is folded into the channel coordinate: offset parity*C of the merged 2C axis).
+    // Box = 64 channels x 16 coarse columns (one padded output line) x 8 coarse rows (the tile's 8 output lines).
+    const int p_ = a->conv_pad;
+    conv_To = (a->conv_T + 2 * p_ - 2) / 2 + 1;
+    conv_Ho = (a->conv_H + 2 * p_ - 2) / 2 + 1;
+    conv_Wo = (a->conv_W + 2 * p_ - 2) / 2 + 1;
+    // odd H / W without padding (SigLIP 27 x 27, stc_connector_v35): the last coarse index would pair the last pixel with
+    // the first one of the next row / frame; no stored output needs it, so it is declared out of bounds (zero fill)
+    const uint64_t wcols = (a->conv_W % 2 == 1 && p_ == 0) ? (uint64_t)a->conv_W / 2 : (uint64_t)(a->conv_W + 1) / 2;
+    const uint64_t hrows = (a->conv_H % 2 == 1 && p_ == 0) ? (uint64_t)a->conv_H / 2 : (uint64_t)(a->conv_H + 1) / 2;
+    const uint64_t C_ = (uint64_t)a->conv_C, W_ = (uint64_t)a->conv_W, H_ = (uint64_t)a->conv_H;
+    uint64_t dims[5] = {2 * C_, wcols, 2, hrows, (uint64_t)a->conv_T};
+    uint64_t str[4] = {2 * C_ * 2, W_ * C_ * 2, 2 * W_ * C_ * 2, H_ * W_ * C_ * 2};
+    uint32_t box[5] = {BK, (uint32_t)kConvLine, 1, (uint32_t)(BM / kConvLine), 1};
+    int rc = make_tmap_bf16(&ta, a->A, 5, dims, str, box);
+    if (rc) return rc;
+  } else {
+    uint64_t dims[2] = {(uint64_t)a->K, (uint64_t)a->M};
+    uint64_t str[1] = {(uint64_t)a->lda * 2};
+    uint32_t box[2] = {BK, BM};
+    int rc = make_tmap_bf16(&ta, a->A, 2, dims, str, box);
+    if (rc) return rc;
+  }
+  {
+    uint64_t dims[2] = {(uint64_t)a->K, (uint64_t)a->N};
+    uint64_t str[1] = {(uint64_t)a->ldw * 2};
+    uint32_t box[2] = {BK, (uint32_t)(PAIR ? BN / 2 : BN)};
+    int rc = make_tmap_bf16(&tb, a->W, 2, dims, str, box);
+    if (rc) return rc;
+  }
+  GemmParams p;
+  p.C = a->C; p.bias = a->bias; p.residual = a->residual; p.row_scale = a->row_scale;
+  p.ldc = a->ldc; p.ldr = a->ldr; p.M = a->M; p.N = a->N; p.K = a->K; p.act = a->act; p.out_f32 = a->out_f32;
+  p.rms_sumsq_in = a->rms_sumsq_in; p.sumsq_out = a->sumsq_out; p.rms_nparts = a->rms_nparts;
+  p.ln_sum_in = a->ln_sum_in; p.ln_colsum = a->ln_colsum; p.rowsum_out = a->rowsum_out;
+  p.rms_inv_dim = a->rms_inv_dim; p.rms_eps = a->rms_eps;
+  p.trace = (a->reserved2 == 777) ? 1 : 0;
+  p.n_bcast = a->n_bcast;
+  p.mc = reinterpret_cast<__nv_bfloat16*>(a->mc_out);
+  for (int i = 0; i < 8; ++i) p.bcast[i] = reinterpret_cast<__nv_bfloat16*>(i < a->n_bcast ? a->bcast_out[i] : nullptr);
+  const int tile_m = PAIR ? 2 * BM : BM;
+  p.rope_tab = a->rope_tab; p.rope_cols = a->rope_cols; p.rope_D = a->rope_D; p.rope_pos0 = a->rope_pos0;
+  p.conv_C = conv ? a->conv_C : 0; p.conv_pad = a->conv_pad; p.conv_Ho = conv_Ho; p.conv_Wo = conv_Wo; p.conv_To = conv_To;
+  const int m_rows = conv ? conv_To * kConvLine * kConvLine : a->M;     // rows of the (padded) A enumeration
+  p.num_m_tiles = (m_rows + tile_m - 1) / tile_m;
+  p.num_n_tiles = (a->N + BN - 1) / BN;
+  const int tiles = p.num_m_tiles * p.num_n_tiles;
+  const int slots = PAIR ? sm_count() / 2 : sm_count();
+  // Split-K of the last, partial round (wave quantisation): the `rem` tiles left for `slots` CTAs (pairs) are cut into s
+  // K-slices each, so the round costs a fraction of a tile time.  Slice 0 owns the tile: it adds the other slices' fp32
+  // partials (workspace, fixed order -> deterministic) and runs the epilogue.  Needs the caller's workspace (splitk_ws).
+  p.split_first = tiles;
+  p.split_s = 1;
+  p.ws_flags = nullptr;
+  p.ws_partial = nullptr;
+  {
+    const int num_kb = (a->K + BK - 1) / BK;
+    const int rem = tiles % slots;
+    // s slices per remaining tile; the rem * s items may need more than one sub-round: pick the s with the shortest tail
+    // ceil(rem * s / slots) / s (in tile times; 1.0 = unsplit).  Items are dealt out in index order, an owner only waits for
+    // higher-numbered items and an item is only queued behind a lower-numbered one, so the waits cannot form a cycle.
+    int s = 1;
+    if (rem > 0) {
+      // a split must beat the unsplit round by 10 % after paying for the partials' round trip through L2
+      const double tile_cycles = kb_cycles(BN, PAIR) * num_kb;
+      double best = 0.9 * tile_cycles;
+      for (int c = 2; c <= 4; ++c) {
+        if (num_kb / c < 8) break;
+        const double tail = (double)((rem * c + slots - 1) / slots) / c;
+        const double cost = tail * tile_cycles + kSplitOverheadCycles;
+        if (cost < best) { best = cost; s = c; }
+      }
+    }
+    const bool forced = rem > 0 && a->reserved3 >= 2 && a->reserved3 <= 4 && num_kb >= a->reserved3;   // test hook
+    if (forced) s = a->reserved3;
+    const size_t need = kSplitFlagBytes + (size_t)rem * (s > 1 ? s - 1 : 0) * tile_m * BN * sizeof(float);
+    if (s > 1 && (splitk_enabled() || forced) && a->splitk_ws != nullptr && (size_t)a->splitk_ws_bytes >= need &&
+        (size_t)2 * rem * kSplitFlagStride * 4 <= kSplitFlagBytes && aligned16(a->splitk_ws)) {
+      p.split_first = tiles - rem;
+      p.split_s = s;
+      p.ws_flags = reinterpret_cast<unsigned*>(a->splitk_ws);
+      p.ws_partial = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(a->splitk_ws) + kSplitFlagBytes);
+    }
+  }
+  p.num_items = p.split_first + (tiles - p.split_first) * p.split_s;
+  const int units = p.num_items < slots ? p.num_items : slots;
+  const dim3 grid(PAIR ? 2 * units : units), block(kGemmThreads);
+  VL2_SMEM_OPT_IN((gemm_bf16_wgmma_kernel<BN, PAIR>), Cfg::kSmemBytes);
+  VL2_CHECK_CUDA(launch_kernel(gemm_bf16_wgmma_kernel<BN, PAIR>, grid, block, Cfg::kSmemBytes, stream, PAIR ? 2 : 1, ta, tb, p));
+  VL2_CHECK_LAUNCH("gemm_bf16_wgmma_kernel");
+  return VL2_OK;
+}
+
+static TileChoice choose_tile(int M, int N, int K, int sms, bool allow_pair, bool allow_split) {
+  const int kb = (K + BK - 1) / BK;
+  static const int cands[7] = {256, 224, 192, 160, 128, 96, 64};
+  TileChoice best = {256, false};
+  double best_cost = -1;
+  for (int pair = (allow_pair ? 1 : 0); pair >= 0; --pair) {
+    for (int i = 0; i < 7; ++i) {
+      const int bn = cands[i];
+      if (pair && bn < 128) continue;
+      if (bn > 64 && N <= bn - 32) continue;  // do not pick a tile much wider than the matrix
+      const int tile_m = pair ? 256 : 128;
+      const long tiles = (long)((M + tile_m - 1) / tile_m) * ((N + bn - 1) / bn);
+      const long slots = pair ? sms / 2 : sms;
+      const long full = tiles / slots, rem = tiles % slots;
+      const double per_kb = kb_cycles(bn, pair != 0);
+      // the last, partial round costs a whole tile time, or a fraction of it when launch_gemm can split it along K
+      double tail = rem > 0 ? 1.0 : 0.0;
+      if (allow_split && rem > 0) {
+        for (int c = 2; c <= 4 && kb / c >= 8; ++c) {
+          const double t = (double)((rem * c + slots - 1) / slots) / c + kSplitOverheadCycles / (per_kb * kb);
+          if (t < tail * 0.9) tail = t;
+        }
+      }
+      const double cost = ((double)full + tail) * (kb * per_kb + 600.0) + 2000.0 + bn * 16.0;
+      if (best_cost < 0 || cost < best_cost * 0.98) { best_cost = cost; best.bn = bn; best.pair = pair != 0; }
+    }
+  }
+  return best;
+}
+
+// VL2_GEMM_SPLITK=1 enables the split-K tail round (needs the caller's workspace).  Default OFF: it makes a GEMM's
+// rounding depend on M (how many tiles land in the last round), which would end the bit-exact frame-sharding /
+// frame-independence properties of the vision tower (tests/test_fullsize_gpu.py).
+static bool splitk_enabled() {
+  static int v = -1;
+  if (v < 0) {
+    const char* e = getenv("VL2_GEMM_SPLITK");
+    v = (e != nullptr && e[0] == '1') ? 1 : 0;
+  }
+  return v == 1;
+}
+
+static bool pair_enabled() {
+  static int v = -1;
+  if (v < 0) {
+    const char* e = getenv("VL2_GEMM_PAIR");
+    v = (e == nullptr || e[0] != '0') ? 1 : 0;
+  }
+  return v == 1;
+}
+
+}  // namespace vl2
+
+// Host-side planning only (no launch, no device work): which tile the cost model picks for a problem and how the
+// persistent grid will be filled.  Lets tests pin the scheduler's decisions for the shapes of the path on a CPU box.
+extern "C" int vl2_gemm_plan(int M, int N, int K, int with_splitk_ws, int32_t* out6) {
+  using namespace vl2;
+  VL2_REQUIRE(M > 0 && N > 0 && K > 0 && out6 != nullptr, VL2_E_BADSHAPE, "vl2_gemm_plan: bad arguments");
+  const int sms = sm_count();
+  const TileChoice t = choose_tile(M, N, K, sms, pair_enabled(), splitk_enabled() && with_splitk_ws != 0);
+  const int tile_m = t.pair ? 2 * BM : BM;
+  const int tiles = ((M + tile_m - 1) / tile_m) * ((N + t.bn - 1) / t.bn);
+  const int slots = t.pair ? sms / 2 : sms;
+  out6[0] = t.bn;
+  out6[1] = t.pair ? 1 : 0;
+  out6[2] = tiles;
+  out6[3] = slots;
+  out6[4] = (tiles + slots - 1) / slots;   // rounds of the persistent loop
+  out6[5] = sms;
+  return VL2_OK;
+}
+
+// Debug: copy the item-boundary cycle trace of the last traced launch (args->reserved2 == 777) to host memory.
+extern "C" int vl2_debug_gemm_trace(long long* host_out128) {
+  VL2_REQUIRE(host_out128 != nullptr, VL2_E_BADSHAPE, "vl2_debug_gemm_trace: null output");
+  VL2_CHECK_CUDA(cudaDeviceSynchronize());
+  VL2_CHECK_CUDA(cudaMemcpyFromSymbol(host_out128, vl2::g_gemm_trace, 128 * sizeof(long long)));
+  return VL2_OK;
+}
+
+extern "C" int vl2_gemm_bf16(const vl2_gemm_args* a, void* stream) {
+  using namespace vl2;
+  VL2_REQUIRE(a != nullptr, VL2_E_BADSHAPE, "vl2_gemm_bf16: null args");
+  VL2_REQUIRE(a->M > 0 && a->N > 0 && a->K > 0, VL2_E_BADSHAPE, "vl2_gemm_bf16: M,N,K must be positive (%d,%d,%d)",
+              a->M, a->N, a->K);
+  VL2_REQUIRE(a->K % 8 == 0 && a->N % 8 == 0, VL2_E_BADSHAPE, "vl2_gemm_bf16: K and N must be multiples of 8 (%d,%d)",
+              a->K, a->N);
+  VL2_REQUIRE(a->lda % 8 == 0 && a->ldw % 8 == 0 && a->ldc % 8 == 0 && (a->residual == nullptr || a->ldr % 8 == 0),
+              VL2_E_BADALIGN, "vl2_gemm_bf16: leading dimensions must be multiples of 8 elements");
+  VL2_REQUIRE(a->lda >= a->K && a->ldw >= a->K, VL2_E_BADSHAPE, "vl2_gemm_bf16: lda/ldw smaller than K");
+  VL2_REQUIRE(aligned16(a->A) && aligned16(a->W) && aligned16(a->C) && aligned16(a->residual) && aligned16(a->bias),
+              VL2_E_BADALIGN, "vl2_gemm_bf16: pointers must be 16-byte aligned");
+  VL2_REQUIRE(a->act >= VL2_ACT_NONE && a->act <= VL2_ACT_GELU_TANH, VL2_E_UNSUPPORTED, "vl2_gemm_bf16: unknown act %d",
+              a->act);
+  VL2_REQUIRE(a->sumsq_out == nullptr || (!a->out_f32 && a->act != VL2_ACT_SWIGLU && a->N % 32 == 0), VL2_E_UNSUPPORTED,
+              "vl2_gemm_bf16: sumsq_out supports bf16, non-SwiGLU outputs with N %% 32 == 0 only");
+  VL2_REQUIRE(a->rms_sumsq_in == nullptr || a->rms_nparts > 0, VL2_E_BADSHAPE, "vl2_gemm_bf16: rms_nparts must be positive");
+  VL2_REQUIRE(a->ln_sum_in == nullptr || (a->rms_sumsq_in != nullptr && a->ln_colsum != nullptr), VL2_E_BADSHAPE,
+              "vl2_gemm_bf16: ln_sum_in needs rms_sumsq_in (sums of squares) and ln_colsum");
+  VL2_REQUIRE(a->rowsum_out == nullptr || a->sumsq_out != nullptr, VL2_E_UNSUPPORTED,
+              "vl2_gemm_bf16: rowsum_out is written together with sumsq_out");
+  VL2_REQUIRE(a->n_bcast >= 0 && a->n_bcast <= 8, VL2_E_BADSHAPE, "vl2_gemm_bf16: n_bcast must be in [0,8]");
+  if (a->n_bcast > 0 || a->mc_out != nullptr) {
+    VL2_REQUIRE(!a->out_f32 && a->act != VL2_ACT_SWIGLU, VL2_E_UNSUPPORTED,
+                "vl2_gemm_bf16: the broadcast epilogue supports bf16, non-SwiGLU outputs only");
+    for (int i = 0; i < a->n_bcast; ++i)
+      VL2_REQUIRE(a->bcast_out[i] != nullptr && aligned16(a->bcast_out[i]), VL2_E_BADALIGN,
+                  "vl2_gemm_bf16: broadcast target %d must be a 16-byte aligned device pointer", i);
+  }
+  if (a->act == VL2_ACT_SWIGLU) {
+    VL2_REQUIRE(a->residual == nullptr && !a->out_f32 && a->N % 16 == 0, VL2_E_UNSUPPORTED,
+                "vl2_gemm_bf16: SWIGLU epilogue needs N %% 16 == 0, bf16 output and no residual");
+  }
+  if (a->rope_tab != nullptr) {
+    VL2_REQUIRE(a->rope_D >= 32 && a->rope_D % 32 == 0 && a->rope_cols > 0 && a->rope_cols % a->rope_D == 0 &&
+                    a->rope_cols <= a->N && a->rope_pos0 >= 0 && aligned16(a->rope_tab),
+                VL2_E_BADSHAPE, "vl2_gemm_bf16: rope epilogue needs head width %% 32 == 0, rope_cols a multiple of it (<= N)");
+    VL2_REQUIRE(!a->out_f32 && a->act == VL2_ACT_NONE && a->residual == nullptr, VL2_E_UNSUPPORTED,
+                "vl2_gemm_bf16: the rope epilogue supports bf16 output without activation / residual");
+  }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  int m_plan = a->M;
+  if (a->conv_C > 0) {
+    const int p_ = a->conv_pad;
+    VL2_REQUIRE(a->conv_T > 0 && a->conv_H > 0 && a->conv_W > 0 && (p_ == 0 || p_ == 1) && a->conv_C % 64 == 0,
+                VL2_E_BADSHAPE, "vl2_gemm_bf16: conv front end needs T,H,W > 0, pad in {0,1}, C %% 64 == 0");
+    const int To = (a->conv_T + 2 * p_ - 2) / 2 + 1, Ho = (a->conv_H + 2 * p_ - 2) / 2 + 1, Wo = (a->conv_W + 2 * p_ - 2) / 2 + 1;
+    VL2_REQUIRE((a->conv_W % 2 == 0 && a->conv_H % 2 == 0) || p_ == 0, VL2_E_UNSUPPORTED,
+                "vl2_gemm_bf16: conv front end: odd H / W needs pad 0");
+    VL2_REQUIRE(To > 0 && Ho > 0 && Wo > 0 && Wo <= kConvLine && Ho <= kConvLine, VL2_E_UNSUPPORTED,
+                "vl2_gemm_bf16: conv front end supports up to %d x %d output positions per time step (got %d x %d)", kConvLine,
+                kConvLine, Ho, Wo);
+    VL2_REQUIRE(a->K == 8 * a->conv_C && a->M == To * Ho * Wo, VL2_E_BADSHAPE,
+                "vl2_gemm_bf16: conv front end needs K == 8*C and M == To*Ho*Wo (M=%d, expected %d)", a->M, To * Ho * Wo);
+    VL2_REQUIRE(a->residual == nullptr && a->row_scale == nullptr && a->rms_sumsq_in == nullptr && a->sumsq_out == nullptr &&
+                    !a->out_f32 && a->act != VL2_ACT_SWIGLU && a->n_bcast == 0 && a->mc_out == nullptr,
+                VL2_E_UNSUPPORTED, "vl2_gemm_bf16: the conv front end supports bias + activation epilogues, bf16 output");
+    m_plan = To * kConvLine * kConvLine;
+  }
+  const bool split_ok = splitk_enabled() && a->splitk_ws != nullptr && a->conv_C == 0;
+  TileChoice t = choose_tile(m_plan, a->N, a->K, sm_count(), pair_enabled(), split_ok);
+  // test hook: reserved = BN forces a single-CTA tile width, 1000 + BN forces the two-CTA (cluster pair) kernel
+  if (a->reserved >= 64 && a->reserved <= 256 && a->reserved % 32 == 0) { t.bn = a->reserved; t.pair = false; }
+  if (a->reserved >= 1128 && a->reserved <= 1256 && (a->reserved - 1000) % 32 == 0) { t.bn = a->reserved - 1000; t.pair = true; }
+  if (t.pair) {
+    switch (t.bn) {
+      case 256: return launch_gemm<256, true>(a, st);
+      case 224: return launch_gemm<224, true>(a, st);
+      case 192: return launch_gemm<192, true>(a, st);
+      case 160: return launch_gemm<160, true>(a, st);
+      default: return launch_gemm<128, true>(a, st);
+    }
+  }
+  switch (t.bn) {
+    case 256: return launch_gemm<256, false>(a, st);
+    case 224: return launch_gemm<224, false>(a, st);
+    case 192: return launch_gemm<192, false>(a, st);
+    case 160: return launch_gemm<160, false>(a, st);
+    case 128: return launch_gemm<128, false>(a, st);
+    case 96: return launch_gemm<96, false>(a, st);
+    default: return launch_gemm<64, false>(a, st);
+  }
+}

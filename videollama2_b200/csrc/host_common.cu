@@ -46,8 +46,8 @@ int sm_count() {
   const int slot = device_slot();
   if (cached[slot] <= 0) {
     int dev = 0, n = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;   // no device: plan for an H100 SXM
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 132;
     cached[slot] = n;
   }
   return cached[slot];

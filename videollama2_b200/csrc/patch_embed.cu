@@ -1,20 +1,19 @@
-// ViT patch embedding as ONE implicit-GEMM kernel on tcgen05 (HF CLIPVisionEmbeddings.forward, HF:clip/modeling_clip.py:202-218,
+// ViT patch embedding as ONE implicit-GEMM kernel on wgmma (HF CLIPVisionEmbeddings.forward, HF:clip/modeling_clip.py:202-218,
 // followed by CLIPVisionTransformer.pre_layrnorm :739-741; HF SiglipVisionEmbeddings for the VideoLLaMA2.1 tower):
 //
 //   tok[f, 1+p, :] = LN( conv_PxP_strideP(pixels[f])[p, :] + pos[1+p, :] ),   tok[f, 0, :] = LN( cls + pos[0, :] )     (CLIP)
 //   tok[f, p, :]   =     conv_PxP_strideP(pixels[f])[p, :] + bias + pos[p, :]                                          (SigLIP)
 //
-// No im2col matrix exists: the A operand (128 patches x K = 3 P^2 pixel values) is gathered from the NCHW frames by 256
-// threads (the 28-byte pixel runs of a 14 x 14 patch break TMA's 16-byte rule, so this is plain LDG) straight into the
-// 128-byte-swizzled shared-memory layout tcgen05.mma reads, once per CTA and for the whole K (10 k-blocks = 160 KB).
-// A 128-patch row block is split along the output channels over a CLUSTER of NS CTAs (NS = 1, 2 or 4; C / NS <= 512
-// columns each), so a 16-frame video fills 144 SMs instead of 72; every CTA keeps its whole column range in TMEM (up to 4
-// accumulators of 128 columns) while the conv weight streams through a 3-stage TMA ring.
-// Epilogue (thread = patch row = TMEM lane): + position row (+ bias).  CLIP: pass 1 reads the accumulators and sums the
-// row's x and x^2 over this CTA's columns; the partial statistics of the NS CTAs are exchanged through distributed shared
-// memory (st.shared::cluster + a remote mbarrier arrive per thread, summed in rank order); pass 2 re-reads TMEM, normalises
-// and stores.  Nothing un-normalised ever leaves the SM.  One launch replaces vl2_patch_im2col + vl2_gemm_bf16 +
-// vl2_clip_embed_finish.
+// No im2col matrix exists: the A operand (128 patches x K = 3 P^2 pixel values) is gathered from the NCHW frames by all
+// threads straight into the 128-byte-swizzled shared-memory layout wgmma reads, once per CTA and for the whole K
+// (10 k-blocks = 160 KB).  A 128-patch row block is split along the output channels over a CLUSTER of NS CTAs
+// (NS <= 8; C / NS <= 256 columns each), so a 16-frame video fills the SMs; each consumer thread keeps its rows' part of
+// the CTA's whole column range in registers (up to two 128-column accumulators) while the conv weight streams through a
+// 2-stage TMA ring.
+// Epilogue: + position row (+ bias).  CLIP: the row's x and x^2 over this CTA's columns (reduced over the quad of threads
+// that hold a row); the partial statistics of the NS CTAs are exchanged through distributed shared memory
+// (st.shared::cluster + remote mbarrier arrives, summed in rank order); then normalise and store.  Nothing un-normalised
+// ever leaves the SM.  One launch replaces vl2_patch_im2col + vl2_gemm_bf16 + vl2_clip_embed_finish.
 #include "host_common.h"
 #include "ptx.cuh"
 #include "row_common.cuh"
@@ -23,9 +22,9 @@ namespace vl2 {
 
 static constexpr int kPeBM = 128, kPeBN = 128, kPeBK = 64;
 static constexpr int kPeMaxKB = 10;                           // K padded to at most 640 (3 * 14 * 14 = 588)
-static constexpr int kPeMaxTiles = 4;                         // 4 x 128 fp32 columns = all 512 TMEM columns
-static constexpr int kPeStagesB = 3;
-static constexpr int kPeThreads = 320;                        // warps 0-3 gather; 4 TMA; 5 MMA; 6-9 gather, then epilogue
+static constexpr int kPeMaxCols = 256;                        // columns per CTA: two 128-column accumulators per thread
+static constexpr int kPeStagesB = 2;
+static constexpr int kPeThreads = 384;                        // warpgroup 0: TMA; 1, 2: wgmma + epilogue; all gather A
 static constexpr int kPeStageB = kPeBN * kPeBK * 2;           // 16 KB
 static constexpr int kPeOffB = kPeMaxKB * kPeBM * kPeBK * 2;  // 160 KB of A
 static constexpr int kPeMaxStatTiles = 16;                    // 128-column tiles of a whole row (C <= 2048 in the LayerNorm form)
@@ -42,7 +41,7 @@ struct PatchEmbedParams {
   const float* bias;            // conv bias (SigLIP) or NULL
   __nv_bfloat16* out;           // [F * (np + has_cls), C]
   int F, H, W, P, G, np, C, K, nkb, M;
-  int ns, cols, n_tiles;        // CTAs per row block (cluster size), columns per CTA, 128-column tiles per CTA
+  int ns, cols, n_tiles;        // CTAs per row block (cluster size), columns per CTA, 128-column B tiles per CTA
   float eps;
 };
 
@@ -60,15 +59,12 @@ patch_embed_kernel(const __grid_constant__ CUtensorMap tmap_w, const PatchEmbedP
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((smem_u32(smem) & 1023u) != 0) { asm volatile("trap;"); }
   uint8_t* sA = smem;                                              // [nkb][128 rows][128 B], swizzled
-  uint8_t* sB = smem + kPeOffB;                                    // [3][128 rows][128 B]
+  uint8_t* sB = smem + kPeOffB;                                    // [2][128 rows][128 B]
   float2* sStats = reinterpret_cast<float2*>(smem + kPeOffStats);  // [global 128-column tile][row] partial (sum, sum of squares)
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kPeOffBar);
-  uint64_t* a_full = bars;            // [10]  gather -> MMA (128 arrivals each)
-  uint64_t* b_full = bars + 10;       // [3]   TMA -> MMA
-  uint64_t* b_empty = bars + 13;      // [3]   MMA -> TMA
-  uint64_t* t_full = bars + 16;       // [4]   MMA -> epilogue, one per accumulator tile
-  uint64_t* stat_bar = bars + 20;     //       128 * ns arrivals: every CTA's partial statistics have landed here
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 21);
+  uint64_t* b_full = bars;            // [2]   TMA -> MMA
+  uint64_t* b_empty = bars + 2;       // [2]   MMA (8 consumer warps) -> TMA
+  uint64_t* stat_bar = bars + 4;      //       64 * ns arrivals: every CTA's partial statistics have landed here
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t rank = p.ns > 1 ? cluster_ctarank() : 0u;
@@ -78,43 +74,32 @@ patch_embed_kernel(const __grid_constant__ CUtensorMap tmap_w, const PatchEmbedP
   const int has_cls = p.cls != nullptr ? 1 : 0;
 
   pdl_launch_dependents();
-  if (warp == 4 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_w);
-    for (int i = 0; i < kPeMaxKB; ++i) mbar_init(&a_full[i], 128);
     for (int i = 0; i < kPeStagesB; ++i) {
       mbar_init(&b_full[i], 1);
-      mbar_init(&b_empty[i], 1);
+      mbar_init(&b_empty[i], 8);
     }
-    for (int i = 0; i < kPeMaxTiles; ++i) mbar_init(&t_full[i], 1);
-    mbar_init(stat_bar, 128 * p.ns);
+    mbar_init(stat_bar, 64 * p.ns);
     fence_barrier_init();
   }
   pdl_wait();
-  if (warp == 5) {
-    tmem_alloc(tmem_ptr, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before_sync();
-  if (p.ns > 1) cluster_sync_all(); else __syncthreads();      // peers' barriers exist before anybody arrives remotely
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_ptr;
-
-  if (warp < 4 || warp >= 6) {
-    // ===================== A gather: 2 threads per patch row (k-blocks [0, nkb/2) and [nkb/2, nkb)) =====================
-    const int half = warp < 4 ? 0 : 1;
-    const int r = (half == 0 ? threadIdx.x : threadIdx.x - 192) & 127;
-    const int m = m0 + r;
-    const bool valid = m < p.M;
-    const int f = valid ? m / p.np : 0, pp = valid ? m % p.np : 0;
-    const int ph = pp / p.G, pw = pp % p.G;
-    const __nv_bfloat16* src0 = p.px + ((int64_t)f * 3 * p.H + (int64_t)ph * p.P) * p.W + pw * p.P;   // (c = 0, i = 0, j = 0)
-    const int64_t cstride = (int64_t)p.H * p.W;
-    const int kb_lo = half == 0 ? 0 : (p.nkb + 1) / 2, kb_hi = half == 0 ? (p.nkb + 1) / 2 : p.nkb;
+  // ===================== A gather by every thread: (patch row, k-block) pairs =====================
+  // The 28-byte pixel runs of a 14 x 14 patch break TMA's 16-byte rule, so this is plain LDG straight into the
+  // 128-byte-swizzled K-major layout wgmma reads.
+  {
     const int pp2 = p.P * p.P;
-    int c = (kb_lo * 64) / pp2, rem = (kb_lo * 64) % pp2;   // decomposition of the running k (advances by 2: P is even)
-    int i = rem / p.P, j = rem % p.P;
-    const uint32_t row_base = smem_u32(sA) + r * 128;
-    for (int kb = kb_lo; kb < kb_hi; ++kb) {
+    const int64_t cstride = (int64_t)p.H * p.W;
+    for (int idx = threadIdx.x; idx < kPeBM * p.nkb; idx += kPeThreads) {
+      const int r = idx & (kPeBM - 1), kb = idx / kPeBM;
+      const int m = m0 + r;
+      const bool valid = m < p.M;
+      const int f = valid ? m / p.np : 0, pp = valid ? m % p.np : 0;
+      const int ph = pp / p.G, pw = pp % p.G;
+      const __nv_bfloat16* src0 = p.px + ((int64_t)f * 3 * p.H + (int64_t)ph * p.P) * p.W + pw * p.P;   // (c = 0, i = 0, j = 0)
+      int c = (kb * 64) / pp2, rem = (kb * 64) % pp2;   // decomposition of the running k (advances by 2: P is even)
+      int i = rem / p.P, j = rem % p.P;
+      const uint32_t row_base = smem_u32(sA) + kb * (kPeBM * 128) + r * 128;
 #pragma unroll
       for (int ch = 0; ch < 8; ++ch) {
         uint32_t w4[4];
@@ -127,149 +112,165 @@ patch_embed_kernel(const __grid_constant__ CUtensorMap tmap_w, const PatchEmbedP
           j += 2;
           if (j == p.P) { j = 0; if (++i == p.P) { i = 0; ++c; } }
         }
-        sts128(row_base + kb * (kPeBM * 128) + ((ch ^ (r & 7)) << 4), make_uint4(w4[0], w4[1], w4[2], w4[3]));
+        sts128(row_base + ((ch ^ (r & 7)) << 4), make_uint4(w4[0], w4[1], w4[2], w4[3]));
       }
-      fence_proxy_async_smem();       // generic-proxy smem writes -> visible to the tensor core's async proxy
-      mbar_arrive(&a_full[kb]);
     }
   }
-  if (warp == 4) {
-    if (lane == 0) {
+  fence_proxy_async_smem();       // generic-proxy smem writes -> visible to the tensor core's async proxy
+  if (p.ns > 1) cluster_sync_all(); else __syncthreads();      // A complete; peers' barriers exist before remote arrivals
+
+  if (warp < 4) {
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
       // ===================== TMA: conv weight tiles [128 output channels x 64 k] of this CTA's column range =====================
-      int g = 0, st = 0;
+      int st = 0;
       uint32_t ph = 0;
       for (int jn = 0; jn < p.n_tiles; ++jn)
-        for (int kb = 0; kb < p.nkb; ++kb, ++g) {
+        for (int kb = 0; kb < p.nkb; ++kb) {
           mbar_wait(&b_empty[st], ph ^ 1);
           mbar_arrive_expect_tx(&b_full[st], kPeStageB);
           tma_load_2d(sB + st * kPeStageB, &tmap_w, &b_full[st], kb * kPeBK, n_begin + jn * kPeBN);
           if (++st == kPeStagesB) { st = 0; ph ^= 1; }
         }
     }
-  } else if (warp == 5) {
-    if (lane == 0) {
-      // ===================== MMA issuer: accumulator tile jn lives at TMEM columns [128 jn, 128 jn + 128) =====================
-      constexpr uint32_t idesc = umma_idesc_bf16(kPeBM, kPeBN, 0, 0);
-      int st = 0;
-      uint32_t ph = 0;
-      for (int jn = 0; jn < p.n_tiles; ++jn) {
-        const uint32_t d_tmem = tmem_base + jn * kPeBN;
-        for (int kb = 0; kb < p.nkb; ++kb) {
-          if (jn == 0) mbar_wait(&a_full[kb], 0);
-          mbar_wait(&b_full[st], ph);
-          tc_fence_after_sync();
-          const uint32_t a_addr = smem_u32(sA) + kb * (kPeBM * 128);
-          const uint32_t b_addr = smem_u32(sB) + st * kPeStageB;
+  } else {
+    setmaxnreg_inc<232>();
+    // ===================== wgmma: accumulator tile jn (columns [128 jn, 128 jn + 128) of the range) =====================
+    const int wg = (warp >> 2) - 1;
+    const int t = lane & 3;
+    const int rloc = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's rows: rloc, rloc + 8
+    const uint64_t da0 = gmma_desc_sw128(smem_u32(sA) + wg * 64 * 128, 16, 1024);
+    const uint64_t db0 = gmma_desc_sw128(smem_u32(sB), 16, 1024);
+    float acc[2][64];
+    int st = 0;
+    uint32_t ph = 0;
 #pragma unroll
-          for (int k = 0; k < kPeBK / 16; ++k)
-            umma_bf16_ss(d_tmem, umma_desc_sw128(a_addr + k * 32, 16, 1024), umma_desc_sw128(b_addr + k * 32, 16, 1024), idesc,
-                         (kb | k) != 0);
-          umma_commit(&b_empty[st]);
-          if (++st == kPeStagesB) { st = 0; ph ^= 1; }
-        }
-        umma_commit(&t_full[jn]);
+    for (int jn = 0; jn < 2; ++jn) {
+      if (jn >= p.n_tiles) break;
+      for (int kb = 0; kb < p.nkb; ++kb) {
+        mbar_wait(&b_full[st], ph);
+        wgmma_fence();
+        const uint64_t da = da0 + (uint64_t)((kb * kPeBM * 128) >> 4);
+        const uint64_t db = db0 + (uint64_t)((st * kPeStageB) >> 4);
+#pragma unroll
+        for (int k = 0; k < kPeBK / 16; ++k) Wgmma<kPeBN, 0>::ss(acc[jn], da + 2 * k, db + 2 * k, (kb | k) != 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_keep(acc[jn]);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&b_empty[st]);
+        if (++st == kPeStagesB) { st = 0; ph ^= 1; }
       }
     }
-  } else if (warp >= 6) {
-    // ===================== epilogue: thread = patch row (TMEM lane) =====================
-    const int q = warp & 3;                            // TMEM lane quarter this warp may read
-    const int r = q * 32 + lane;
-    const int m = m0 + r;
-    const bool valid = m < p.M;
-    const int f = valid ? m / p.np : 0, pp = valid ? m % p.np : 0;
-    const int64_t out_row = (int64_t)f * (p.np + has_cls) + has_cls + pp;
-    const __nv_bfloat16* pos_row = p.pos + (int64_t)(has_cls + pp) * p.C + n_begin;
-    const uint32_t lane_sel = (uint32_t)(q * 32) << 16;
-    const int n_chunks = p.cols / 32;
-
-    // x of one 32-column chunk: accumulator (+ bias) + position row, exactly as both passes must see it
-    auto load_chunk = [&](int ck, float (&x)[32]) {
-      uint32_t v[32];
-      tmem_ld_32x32(tmem_base + lane_sel + ck * 32, v);
-      uint4 pv[4];
+    // ===================== epilogue.  acc[jn][4 c + 2 h + e] = row rloc + 8 h, column 128 jn + 8 c + 2 t + e =====================
+    int out_row[2];
+    bool valid[2];
+    const __nv_bfloat16* pos_row[2];
 #pragma unroll
-      for (int g = 0; g < 4; ++g) pv[g] = valid ? __ldg(reinterpret_cast<const uint4*>(pos_row + ck * 32) + g) : make_uint4(0, 0, 0, 0);
-      tmem_ld_wait();
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        float pf[8];
-        unpack8(pv[g], pf);
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          const float a = __uint_as_float(v[g * 8 + e]);
-          // CLIP: the conv output is rounded to 16 bits (HF's conv returns the activation dtype) before the fp32 position
-          // add + LayerNorm; SigLIP: conv + bias + position in fp32, one rounding at the store
-          x[g * 8 + e] = clip ? __bfloat162float(__float2bfloat16_rn(a)) + pf[e]
-                              : a + (p.bias != nullptr ? __ldg(p.bias + n_begin + ck * 32 + g * 8 + e) : 0.f) + pf[e];
-        }
+    for (int h = 0; h < 2; ++h) {
+      const int m = m0 + rloc + 8 * h;
+      valid[h] = m < p.M;
+      const int f = valid[h] ? m / p.np : 0, pp = valid[h] ? m % p.np : 0;
+      out_row[h] = f * (p.np + has_cls) + has_cls + pp;
+      pos_row[h] = p.pos + (int64_t)(has_cls + pp) * p.C + n_begin;
+    }
+    // x of one column pair: accumulator (+ bias) + position row, exactly as both passes must see it
+    auto load_pair = [&](int jn, int c, int h, float& x0, float& x1) {
+      const int col = jn * kPeBN + 8 * c + 2 * t;
+      const uint32_t pv = valid[h] ? __ldg(reinterpret_cast<const uint32_t*>(pos_row[h] + col)) : 0u;
+      const float a0 = acc[jn][4 * c + 2 * h], a1 = acc[jn][4 * c + 2 * h + 1];
+      // CLIP: the conv output is rounded to 16 bits (HF's conv returns the activation dtype) before the fp32 position
+      // add + LayerNorm; SigLIP: conv + bias + position in fp32, one rounding at the store
+      if (clip) {
+        x0 = __bfloat162float(__float2bfloat16_rn(a0)) + bf16_lo(pv);
+        x1 = __bfloat162float(__float2bfloat16_rn(a1)) + bf16_hi(pv);
+      } else {
+        const float2 bq = p.bias != nullptr ? __ldg(reinterpret_cast<const float2*>(p.bias + n_begin + col)) : make_float2(0.f, 0.f);
+        x0 = a0 + bq.x + bf16_lo(pv);
+        x1 = a1 + bq.y + bf16_hi(pv);
       }
     };
-    auto store_chunk = [&](int ck, const float (&x)[32]) {
-      __nv_bfloat16* orow = p.out + out_row * p.C + n_begin + ck * 32;
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        float o8[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) o8[e] = x[g * 8 + e];
-        *reinterpret_cast<uint4*>(orow + g * 8) = pack8(o8);
-      }
-    };
-
-    float mean = 0.f, rstd = 1.f;
+    float mean[2] = {0.f, 0.f}, rstd[2] = {1.f, 1.f};
     if (clip) {
-      // ---- pass 1: the row statistics of this CTA's columns, ONE partial per 128-column tile.  The tiles are the same
-      // whatever the cluster size (column ranges are multiples of 128 whenever the split can vary), and the final sum below
-      // runs over the row's tiles in global order: the result does not depend on how many CTAs shared the row, which keeps
-      // the tower bit-identical for any number of frames per launch (frame sharding).
+      // ---- the row statistics of this CTA's columns, ONE partial per 128-column tile.  The tiles are the same whatever
+      // the cluster size (column ranges are multiples of 128 whenever the split can vary), and the final sum below runs
+      // over the row's tiles in global order: the result does not depend on how many CTAs shared the row, which keeps the
+      // tower bit-identical for any number of frames per launch (frame sharding).
       const int tile0 = n_begin / kPeBN;
-      for (int jn = 0; jn < p.n_tiles; ++jn) {
-        mbar_wait(&t_full[jn], 0);
-        tc_fence_after_sync();
-        float s = 0.f, sq = 0.f;
-        for (int ck = jn * 4; ck < min(n_chunks, jn * 4 + 4); ++ck) {
-          float x[32];
-          load_chunk(ck, x);
 #pragma unroll
-          for (int e = 0; e < 32; ++e) { s += x[e]; sq = fmaf(x[e], x[e], sq); }
-        }
-        // ---- hand the partial to every CTA of the cluster (distributed shared memory)
-        const uint32_t slot = smem_u32(sStats + (tile0 + jn) * 128 + r);
-        if (p.ns > 1) {
-          for (uint32_t rr = 0; rr < (uint32_t)p.ns; ++rr) st_cluster_f32x2(slot, rr, s, sq);
-        } else {
-          sStats[(tile0 + jn) * 128 + r] = make_float2(s, sq);
+      for (int jn = 0; jn < 2; ++jn) {
+        if (jn >= p.n_tiles) break;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float s = 0.f, sq = 0.f;
+#pragma unroll
+          for (int c = 0; c < 16; ++c) {
+            if (jn * kPeBN + 8 * c >= p.cols) break;
+            float x0, x1;
+            load_pair(jn, c, h, x0, x1);
+            s += x0 + x1;
+            sq = fmaf(x0, x0, fmaf(x1, x1, sq));
+          }
+          s += __shfl_xor_sync(0xffffffffu, s, 1);
+          s += __shfl_xor_sync(0xffffffffu, s, 2);
+          sq += __shfl_xor_sync(0xffffffffu, sq, 1);
+          sq += __shfl_xor_sync(0xffffffffu, sq, 2);
+          // ---- hand the partial to every CTA of the cluster (distributed shared memory)
+          const int r = rloc + 8 * h;
+          if (t == 0) {
+            if (p.ns > 1) {
+              const uint32_t slot = smem_u32(sStats + (tile0 + jn) * 128 + r);
+              for (uint32_t rr = 0; rr < (uint32_t)p.ns; ++rr) st_cluster_f32x2(slot, rr, s, sq);
+            } else {
+              sStats[(tile0 + jn) * 128 + r] = make_float2(s, sq);
+            }
+          }
         }
       }
-      for (uint32_t rr = 0; rr < (uint32_t)p.ns; ++rr) {
-        if (p.ns > 1) mbar_arrive_cluster(stat_bar, rr);   // release.cluster: the stores above are visible to whoever acquires
-        else mbar_arrive(stat_bar);
+      if (t == 0) {
+        for (uint32_t rr = 0; rr < (uint32_t)p.ns; ++rr) {
+          if (p.ns > 1) mbar_arrive_cluster(stat_bar, rr);   // release.cluster: the stores above are visible to whoever acquires
+          else mbar_arrive(stat_bar);
+        }
       }
       mbar_wait_cluster(stat_bar, 0);                // acquire.cluster: pairs with the peers' release arrivals
-      float ts = 0.f, tq = 0.f;
       const int row_tiles = (p.C + kPeBN - 1) / kPeBN;
-      for (int t = 0; t < row_tiles; ++t) { const float2 v2 = sStats[t * 128 + r]; ts += v2.x; tq += v2.y; }
-      mean = ts / (float)p.C;
-      rstd = rsqrtf(fmaxf(tq / (float)p.C - mean * mean, 0.f) + p.eps);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float ts = 0.f, tq = 0.f;
+        for (int tt = 0; tt < row_tiles; ++tt) { const float2 v2 = sStats[tt * 128 + rloc + 8 * h]; ts += v2.x; tq += v2.y; }
+        mean[h] = ts / (float)p.C;
+        rstd[h] = rsqrtf(fmaxf(tq / (float)p.C - mean[h] * mean[h], 0.f) + p.eps);
+      }
     }
-    // ---- pass 2 (the only pass without a LayerNorm): normalise / finish and store
-    for (int ck = 0; ck < n_chunks; ++ck) {
-      if (!clip && (ck & 3) == 0) { mbar_wait(&t_full[ck >> 2], 0); tc_fence_after_sync(); }
-      float x[32];
-      load_chunk(ck, x);
-      if (clip) {
+    // ---- normalise / finish and store
 #pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          float gm[8], bt[8];
-          unpack8(__ldg(reinterpret_cast<const uint4*>(p.gamma + n_begin + ck * 32) + g), gm);    // same address in every lane
-          unpack8(__ldg(reinterpret_cast<const uint4*>(p.beta + n_begin + ck * 32) + g), bt);
+    for (int jn = 0; jn < 2; ++jn) {
+      if (jn >= p.n_tiles) break;
 #pragma unroll
-          for (int e = 0; e < 8; ++e) x[g * 8 + e] = (x[g * 8 + e] - mean) * rstd * gm[e] + bt[e];
+      for (int c = 0; c < 16; ++c) {
+        const int col = jn * kPeBN + 8 * c + 2 * t;
+        if (jn * kPeBN + 8 * c >= p.cols) break;
+        float gm0 = 1.f, gm1 = 1.f, bt0 = 0.f, bt1 = 0.f;
+        if (clip) {
+          const uint32_t gv = __ldg(reinterpret_cast<const uint32_t*>(p.gamma + n_begin + col));
+          const uint32_t bv = __ldg(reinterpret_cast<const uint32_t*>(p.beta + n_begin + col));
+          gm0 = bf16_lo(gv); gm1 = bf16_hi(gv); bt0 = bf16_lo(bv); bt1 = bf16_hi(bv);
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float x0, x1;
+          load_pair(jn, c, h, x0, x1);
+          if (clip) {
+            x0 = (x0 - mean[h]) * rstd[h] * gm0 + bt0;
+            x1 = (x1 - mean[h]) * rstd[h] * gm1 + bt1;
+          }
+          if (valid[h]) *reinterpret_cast<uint32_t*>(p.out + (int64_t)out_row[h] * p.C + n_begin + col) = pack_bf16(x0, x1);
         }
       }
-      if (valid) store_chunk(ck, x);
     }
     // the class-token row is the same for every frame: LN(cls + pos[0]); the CTAs of row block 0 write their column range
-    if (clip && m0 == 0 && q == 0) {
+    if (clip && m0 == 0 && warp == 4) {
       float cs = 0.f, cq = 0.f;
       for (int c0 = lane * 8; c0 < p.C; c0 += 256) {
         float a[8], b[8];
@@ -295,13 +296,7 @@ patch_embed_kernel(const __grid_constant__ CUtensorMap tmap_w, const PatchEmbedP
       }
     }
   }
-
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 512);
-  }
+  if (p.ns > 1) cluster_sync_all();   // no CTA leaves while a peer may still write its statistics into it
 }
 
 }  // namespace vl2
@@ -330,23 +325,24 @@ extern "C" int vl2_patch_embed(const vl2_patch_embed_args* a, void* stream) {
   p.out = (__nv_bfloat16*)a->out;
   p.F = a->F; p.H = a->H; p.W = a->W; p.P = a->P; p.G = a->W / a->P; p.np = (a->H / a->P) * (a->W / a->P); p.C = a->C;
   p.K = K; p.nkb = a->Kpad / 64; p.M = a->F * p.np; p.eps = a->eps;
-  // Columns per CTA: at most 512 (TMEM), a multiple of 32 (epilogue chunks); prefer the split that fills the SMs.  The
-  // split is a cluster of 1, 2 or 4 CTAs (the CLIP form exchanges LayerNorm statistics over it); 3 suits SigLIP's 1152.
+  // Columns per CTA: at most 256 (two 128-column register accumulators per consumer thread), a multiple of 32; prefer the
+  // split that fills the SMs.  The split is a cluster of up to 8 CTAs (the CLIP form exchanges LayerNorm statistics over
+  // it, so its column ranges are whole 128-column tiles); 3 and 6 suit SigLIP's 1152 and 288-wide test towers.
   const int blocks_m = (p.M + kPeBM - 1) / kPeBM;
   int ns = 0;
-  const int cands_clip[3] = {1, 2, 4}, cands_any[4] = {1, 2, 3, 4};
+  const int cands_clip[4] = {1, 2, 4, 8}, cands_any[6] = {1, 2, 3, 4, 6, 8};
   const int* cands = clip ? cands_clip : cands_any;
-  const int ncand = clip ? 3 : 4;
+  const int ncand = clip ? 4 : 6;
   for (int i = 0; i < ncand; ++i) {
     const int s = cands[i];
-    if (a->C % s != 0 || (a->C / s) % 32 != 0 || a->C / s > kPeMaxTiles * kPeBN) continue;
+    if (a->C % s != 0 || (a->C / s) % 32 != 0 || a->C / s > kPeMaxCols) continue;
     if (clip && s > 1 && (a->C / s) % kPeBN != 0) continue;            // statistics tiles must line up with global 128-column tiles
     if (ns == 0) ns = s;
     else if (blocks_m * s <= sm_count() && a->C / s >= 128) ns = s;      // a finer split only while it still is one wave
   }
   VL2_REQUIRE(!clip || (a->C + kPeBN - 1) / kPeBN <= kPeMaxStatTiles, VL2_E_UNSUPPORTED, "vl2_patch_embed: C <= %d with a LayerNorm",
               kPeMaxStatTiles * kPeBN);
-  VL2_REQUIRE(ns > 0, VL2_E_UNSUPPORTED, "vl2_patch_embed: C = %d cannot be split into <= 4 column ranges of <= 512", a->C);
+  VL2_REQUIRE(ns > 0, VL2_E_UNSUPPORTED, "vl2_patch_embed: C = %d cannot be split into <= 8 column ranges of <= 256", a->C);
   p.ns = ns; p.cols = a->C / ns; p.n_tiles = (p.cols + kPeBN - 1) / kPeBN;
   CUtensorMap tw;
   {

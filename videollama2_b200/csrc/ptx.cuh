@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA / TMEM / commit).
-// Everything here is device-only and header-only; used by gemm_tcgen05.cu and attn_tcgen05.cu.
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), clusters, wgmma (see also wgmma.cuh).
+// Everything here is device-only and header-only.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -12,7 +12,7 @@
 // libvl2_f16.so (-DVL2_HALF) as IEEE fp16 - the reference's own inference dtype (videollama2/__init__.py:60,
 // model/__init__.py:71 load everything with torch_dtype=float16).  Every kernel moves 16-bit elements through the helpers
 // below (pack_bf16 / bf16_lo / bf16_hi / unpack8 / pack8) and the CUDA conversion intrinsics, so the half build only
-// re-targets those names; accumulation is fp32 either way and tcgen05.mma kind::f16 takes both input formats.
+// re-targets those names; accumulation is fp32 either way and wgmma takes both input formats.
 // ----------------------------------------------------------------------------------------------
 #ifdef VL2_HALF
 #define __nv_bfloat16 __half
@@ -21,12 +21,12 @@
 #define __bfloat162float __half2float
 #define __floats2bfloat162_rn __floats2half2_rn
 #define __bfloat16_as_ushort __half_as_ushort
-#define VL2_UMMA_FMT 0u                          // tcgen05 instruction descriptor: A / B format F16
+#define VL2_WGMMA_TYPES "f16.f16"
 #define VL2_MMA_SYNC_TYPES "f16.f16"
 #define VL2_MULTIMEM_TYPE "f16x2"
 #define VL2_STORAGE_DTYPE 1
 #else
-#define VL2_UMMA_FMT 1u                          // BF16
+#define VL2_WGMMA_TYPES "bf16.bf16"
 #define VL2_MMA_SYNC_TYPES "bf16.bf16"
 #define VL2_MULTIMEM_TYPE "bf16x2"
 #define VL2_STORAGE_DTYPE 0
@@ -157,17 +157,12 @@ __device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity
   }
 }
 
+
 // ----------------------------------------------------------------------------------------------
-// Proxy / tcgen05 fences
+// Proxy fence: generic-proxy shared-memory writes -> visible to the async proxy (TMA, wgmma operands)
 // ----------------------------------------------------------------------------------------------
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_before_sync() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after_sync() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -237,127 +232,19 @@ __device__ __forceinline__ void tma_load_5d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
-// ----------------------------------------------------------------------------------------------
-// TMEM allocation (one full warp executes these)
-// ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// ----------------------------------------------------------------------------------------------
-// UMMA descriptors.
-//
-// Shared-memory matrix descriptor (64 bit), sm_100 flavour:
-//   [0,14)  start address >> 4        [16,30) leading-dim byte offset >> 4
-//   [32,46) stride-dim byte offset >> 4   [46,48) version = 1   [49,52) base offset   [61,64) layout type
-// layout type: 0 none, 1 128B_base32B, 2 128B, 4 64B, 6 32B.
-//
-// K-major, SWIZZLE_128B (what TMA writes for a {64 x rows} bf16 box with CU_TENSOR_MAP_SWIZZLE_128B):
-//   row r lives at r*128 B, its 16-byte chunks XOR-ed with (r & 7); 8-row groups are 1024 B apart => SBO = 1024.
-//   LBO is ignored for swizzled K-major layouts (set to 1).  Stepping K by 16 bf16 inside the 128-B atom is
-//   start_address += 32 B.
-// MN-major, SWIZZLE_128B (a {64 x k-rows} box whose contiguous dim is M/N):
-//   element (mn, k) lives at k*128 B + mn*2 B (swizzled by k & 7); 8-k groups 1024 B apart => SBO = 1024;
-//   the next 64-wide MN atom is LBO bytes away.  Stepping K by 16 is start_address += 2048 B.
-// ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;  // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;  // SWIZZLE_128B
-  return d;
-}
-
-// The same descriptor as two 32-bit words.  The start address lives in bits [0,14) of the LOW word, so stepping through a
-// tile is `lo + (byte_offset >> 4)` (no carry out of the field while the address stays inside the 228 KB of shared memory)
-// and the high word is a compile-time constant: an issuing thread that keeps (lo, hi) apart needs ONE uniform add per
-// operand per MMA, where rebuilding the 64-bit descriptor from the address costs a dependent shift / mask / or chain of
-// uniform-datapath instructions (~100 cycles per tcgen05.mma, measured in the attention kernel's timeline trace).
-__host__ __device__ constexpr uint32_t umma_desc_sw128_hi(uint32_t sbo_bytes) {
-  return ((sbo_bytes >> 4) & 0x3FFF) | (1u << 14) | (2u << 29);
-}
-__device__ __forceinline__ uint32_t umma_desc_sw128_lo(uint32_t smem_addr, uint32_t lbo_bytes) {
-  return ((smem_addr >> 4) & 0x3FFF) | (((lbo_bytes >> 4) & 0x3FFF) << 16);
-}
-// D[tmem] (+)= A[smem] * B[smem] with the descriptors given as (lo, hi) words; issued by ONE (elected) thread.
-__device__ __forceinline__ void umma_bf16_ss_lohi(uint32_t d_tmem, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi,
-                                                  uint32_t idesc, uint32_t accumulate) {
+// TMA load of one box, written to the same shared-memory offset in every CTA of `cta_mask` (cluster multicast); each
+// destination CTA's mbarrier at the offset of `bar` receives the bytes it got.
+__device__ __forceinline__ void tma_load_2d_mc(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
+                                               uint16_t cta_mask) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "mov.b64 da, {%1, %2};\n\t"
-      "mov.b64 db, {%3, %4};\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t}\n"
-      ::"r"(d_tmem), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
+      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
       : "memory");
 }
 
-// cta_group::2 form of the same (leader CTA's elected thread; operands from both CTAs' shared memory)
-__device__ __forceinline__ void umma_bf16_ss_pair_lohi(uint32_t d_tmem, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi,
-                                                       uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "mov.b64 da, {%1, %2};\n\t"
-      "mov.b64 db, {%3, %4};\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], da, db, %5, p;\n\t}\n"
-      ::"r"(d_tmem), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]: the A operand (M = 128 rows = TMEM lanes, K along the columns, two 16-bit elements
-// per 32-bit column: element k in column k / 2, even k in the low half) is read from tensor memory - no shared-memory
-// traffic for it.  Issued by ONE (elected) thread.
-__device__ __forceinline__ void umma_bf16_ts_lohi(uint32_t d_tmem, uint32_t a_tmem, uint32_t b_lo, uint32_t b_hi, uint32_t idesc,
-                                                  uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 db;\n\t"
-      "setp.ne.b32 p, %5, 0;\n\t"
-      "mov.b64 db, {%2, %3};\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], db, %4, p;\n\t}\n"
-      ::"r"(d_tmem), "r"(a_tmem), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// Instruction descriptor for kind::f16 with BF16 A/B and FP32 accumulate.
-//   [4,6) c_format (1 = f32)  [7,10) a_format (1 = bf16)  [10,13) b_format  [15] a_major  [16] b_major
-//   [17,23) N >> 3   [24,29) M >> 4
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (VL2_UMMA_FMT << 7) | (VL2_UMMA_FMT << 10) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread.
-__device__ __forceinline__ void umma_bf16_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// ---- cta_group::2 (CTA pair) variants --------------------------------------------------------------------------
-// Shared addresses of a clustered launch carry the CTA rank in bit 24; clearing it addresses the same offset in the
-// even ("leader") CTA of the pair (CUTLASS: Sm100MmaPeerBitMask).
-static constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-
+// ----------------------------------------------------------------------------------------------
+// Clusters
+// ----------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -365,29 +252,6 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
 }
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// TMA load whose completion bytes are credited to the LEADER CTA's mbarrier (executed by both CTAs of the pair)
-__device__ __forceinline__ void tma_load_2d_pair(void* smem_dst, const CUtensorMap* m, uint64_t* bar_local, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar_local) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_pair(void* smem_dst, const CUtensorMap* m, uint64_t* bar_local, int c0, int c1,
-                                                 int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], "
-      "[%2];" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar_local) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_5d_pair(void* smem_dst, const CUtensorMap* m, uint64_t* bar_local, int c0, int c1,
-                                                 int c2, int c3, int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], "
-      "[%2];" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar_local) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-      : "memory");
 }
 // arrive on the barrier at the same smem offset in CTA `rank` of the cluster
 __device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar_local, uint32_t rank) {
@@ -398,78 +262,44 @@ __device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar_local, uint32_
       ::"r"(smem_u32(bar_local)), "r"(rank)
       : "memory");
 }
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_pair() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem of both CTAs] (+)= A (128 rows from each CTA's smem) * B (N/2 rows from each CTA's smem); leader thread only
-__device__ __forceinline__ void umma_bf16_ss_pair(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                                  uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// commit -> arrive on the barrier at this smem offset in BOTH CTAs of the pair
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar_local) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(smem_u32(bar_local) & kPeerBitMask), "h"((uint16_t)3)
-      : "memory");
-}
 
-// TMEM -> registers: each thread of the warp reads 32 consecutive fp32 columns of its own lane
-// (lane = 32 * (warp_id % 4) + lane_id).  taddr = (lane << 16) | column.
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// registers -> TMEM, same 32x32b shape (thread writes 32 consecutive columns of its lane)
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};\n"
-      ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]),
-        "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]),
-        "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]),
-        "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-// the same store, 16 columns
-__device__ __forceinline__ void tmem_st_32x32_x16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};\n"
-      ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]),
-        "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// three-input maximum (one FMNMX3 on sm_100)
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
+// ----------------------------------------------------------------------------------------------
+// Warpgroup MMA (wgmma).  Shared-memory matrix descriptor (64 bit), sm_90 flavour:
+//   [0,14) start address >> 4   [16,30) leading-dim byte offset >> 4   [32,46) stride-dim byte offset >> 4
+//   [49,52) base offset          [62,64) layout type (1 = 128B swizzle)
+// K-major, SWIZZLE_128B (what TMA writes for a {64 x rows} 16-bit box with CU_TENSOR_MAP_SWIZZLE_128B):
+//   row r lives at r*128 B, its 16-byte chunks XOR-ed with (r & 7); 8-row groups are 1024 B apart => SBO = 1024;
+//   LBO is unused.  Stepping K by 16 elements inside the 128-B atom is start address += 32 B.
+// MN-major, SWIZZLE_128B (a {64 x k-rows} box whose contiguous dim is M/N):
+//   element (mn, k) lives at k*128 B + mn*2 B (swizzled by k & 7); 8-k groups 1024 B apart => SBO = 1024;
+//   the next 64-wide MN atom is LBO bytes away.  Stepping K by 16 is start address += 2048 B.
+// Stage bases are 1024-byte aligned, so the base offset field stays 0.
+// ----------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
+  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
+  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
+  d |= (uint64_t)1 << 62;  // SWIZZLE_128B
   return d;
 }
+// order this thread's register / shared-memory accesses before the wgmma that follow (accumulators, register A operands)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// wait until at most N committed wgmma groups of this warpgroup are still in flight
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keep the compiler from moving accumulator reads / writes across a wgmma that is still in flight
+template <int N>
+__device__ __forceinline__ void wgmma_keep(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// register budget of a warpgroup role (all warps of the warpgroup execute it)
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // 2^x on the MUFU pipe (single instruction; inputs here are <= ~8, flush-to-zero is fine for probabilities)
 __device__ __forceinline__ float fast_exp2(float x) {
@@ -509,3 +339,5 @@ __device__ __forceinline__ float bf16_hi(uint32_t u) { return __uint_as_float(u 
 #endif
 
 }  // namespace vl2
+
+#include "wgmma.cuh"

@@ -57,7 +57,7 @@ __device__ __forceinline__ void multimem_st_f32(float* mc_addr, float v) {
   asm volatile("multimem.st.relaxed.sys.global.f32 [%0], %1;" ::"l"(mc_addr), "f"(v) : "memory");
 }
 
-// RED_MC: reduce inside the NVSwitch (multimem.ld_reduce).  Measured on B200 (scripts/tp_allreduce_check.py): the switch does
+// RED_MC: reduce inside the NVSwitch (multimem.ld_reduce).  Checked with scripts/tp_allreduce_check.py: the switch does
 // NOT round the bf16 result to nearest - ~19 % of the elements differ by one bf16 ulp from the correctly rounded fp32 sum
 // (which NCCL and the peer-load path both produce bit for bit) - so it is opt-in; the default reduces with peer loads in
 // rank order (exact fp32 accumulation, one rounding) and uses the switch only to BROADCAST (ST_MC: multimem.st, an exact copy).

@@ -91,9 +91,9 @@ def load_pretrained_model(model_path, model_base=None, model_name=None, load_8bi
     base + `mm_projector.bin` branch (:138-164); returns (tokenizer, model, image_processor, context_len).  LoRA / 4-bit /
     8-bit branches are training artefacts outside the accelerated path."""
     if load_8bit or load_4bit:
-        raise NotImplementedError("bitsandbytes loading is not supported by the B200 engine")
+        raise NotImplementedError("bitsandbytes loading is not supported by this engine")
     if model_name and "lora" in model_name.lower():
-        raise NotImplementedError("LoRA-adapter loading is not supported by the B200 engine (merge the adapter first)")
+        raise NotImplementedError("LoRA-adapter loading is not supported by this engine (merge the adapter first)")
     with open(os.path.join(model_path, "config.json")) as fh:
         raw = json.load(fh)
     model_type = raw.get("model_type", "videollama2_mistral")

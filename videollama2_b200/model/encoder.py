@@ -95,7 +95,7 @@ class CLIPVisionTower:
         D = C // H
         S = self.num_patches + 1
         if self.fused_embed and self.kpad <= 640 and c.patch_size % 2 == 0 and C % 32 == 0:
-            # one implicit-GEMM launch: gather patches -> tcgen05 conv -> + position -> class row -> pre-LayerNorm
+            # one implicit-GEMM launch: gather patches -> wgmma conv -> + position -> class row -> pre-LayerNorm
             x = ops.patch_embed(images.contiguous(), self.w["patch"], self.w["pos"], c.patch_size, cls=self.w["cls"],
                                 gamma=self.w["pre_g"], beta=self.w["pre_b"], eps=c.layer_norm_eps)
         else:
@@ -110,10 +110,9 @@ class CLIPVisionTower:
 
     # LayerNorms folded into the GEMMs that consume them (VL2_VIT_FOLD_LN=1): gamma goes into the weight columns, beta into
     # the bias, and the row statistics (sum, sum of squares) come out of the epilogue of the GEMM that produced the residual
-    # stream - 2 launches and 2 round trips of the stream fewer per layer.  Parity-tested, but OFF by default: measured on
-    # B200 (profiles/r02_vit_shard_probe.json) the K = 1024 tower GEMMs are epilogue-bound, so the extra epilogue work costs
-    # more than the 46 stand-alone LayerNorm launches it removes at 8-16 frames (8.22 vs 7.71 ms) and only pays at 2 frames
-    # per GPU (2.51 vs 2.61 ms).
+    # stream - 2 launches and 2 round trips of the stream fewer per layer.  Parity-tested, but OFF by default: the K = 1024 tower
+    # GEMMs are epilogue-bound, so the extra epilogue work can cost more than the 46 stand-alone LayerNorm launches it
+    # removes (not measured on the H100).
     fold_layernorm = os.environ.get("VL2_VIT_FOLD_LN", "0") == "1"
     # embeddings as ONE implicit-GEMM kernel (vl2_patch_embed); VL2_VIT_FUSED_EMBED=0 -> explicit im2col + GEMM + finish
     fused_embed = os.environ.get("VL2_VIT_FUSED_EMBED", "1") != "0"
@@ -308,7 +307,7 @@ class SiglipVisionTower(CLIPVisionTower):
     def hidden_states(self, images: torch.Tensor, last_out: Optional[torch.Tensor] = None, bcast_ptrs=None,
                       mc_ptr: int = 0) -> torch.Tensor:
         """[F,3,H,W] bf16 -> residual stream after the selected layer, [F, np, C].  The embedding is ONE implicit-GEMM
-        launch (vl2_patch_embed: patches gathered from the frames, conv on tcgen05, + bias + position rows in the epilogue);
+        launch (vl2_patch_embed: patches gathered from the frames, conv on wgmma, + bias + position rows in the epilogue);
         the explicit form (im2col + GEMM with the position table as residual operand) remains for the folded-LN variant."""
         c = self._config
         Fn = images.shape[0]

@@ -210,7 +210,7 @@ class STCConnectorV35(STCConnector):
 
 
 def build_vision_projector(config, delay_load=False, **kwargs):
-    """projector.py:95-122.  The B200 engine implements the STC family; the ablation variants are not on the hot path."""
+    """projector.py:95-122.  This engine implements the STC family; the ablation variants are not on the hot path."""
     projector_type = getattr(config, "mm_projector_type", "linear")
     if projector_type == "stc_connector":
         return STCConnector(config)
@@ -218,5 +218,5 @@ def build_vision_projector(config, delay_load=False, **kwargs):
         return STCConnectorV35(config)
     if projector_type in ("linear", "identity", "stp_connector", "spatial_conv", "spatial_pool") or \
             re.match(r"^mlp(\d+)x_gelu$", projector_type):
-        raise NotImplementedError(f"projector type {projector_type} is not implemented in the B200 engine")
+        raise NotImplementedError(f"projector type {projector_type} is not implemented in this engine")
     raise ValueError(f"Unknown projector type: {projector_type}")

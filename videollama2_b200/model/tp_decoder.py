@@ -1,4 +1,4 @@
-"""Tensor-parallel decoder for the 72B configuration (BASELINE.json configs[4]: VideoLLaMA2-72B = Qwen2-72B backbone, 8 x B200).
+"""Tensor-parallel decoder for the 72B configuration (BASELINE.json configs[4]: VideoLLaMA2-72B = Qwen2-72B backbone, 8 GPUs).
 
 The reference has no tensor parallelism: its only multi-GPU loading is `device_map="auto"` (videollama2/model/__init__.py:48,54,
 layer-wise placement by accelerate); 150 GB of bf16 weights need the 8 GPUs of a box either way.  This engine shards every

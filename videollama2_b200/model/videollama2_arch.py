@@ -156,7 +156,7 @@ class Videollama2MetaForCausalLM:
         if "tc_connector" in ptype or "tp_connector" in ptype or ptype in ("spatial_conv", "spatial_pool"):
             return self.get_model().mm_projector(frames_features)
         if ptype in ("mlp2x_gelu", "linear"):
-            raise NotImplementedError(f"projector type {ptype} is not implemented in the B200 engine")
+            raise NotImplementedError(f"projector type {ptype} is not implemented in this engine")
         raise Exception(f"Unsupported projector type {ptype}!!!")
 
     # arch.py:161-263

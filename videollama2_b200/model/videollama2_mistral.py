@@ -1,5 +1,5 @@
 """Videollama2MistralForCausalLM with the reference's call surface (videollama2/model/videollama2_mistral.py:47-153),
-backed by the B200 engine instead of HF MistralForCausalLM."""
+backed by the H100 engine instead of HF MistralForCausalLM."""
 from __future__ import annotations
 
 from types import SimpleNamespace

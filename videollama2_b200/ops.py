@@ -79,7 +79,7 @@ def gemm(a: torch.Tensor, w: torch.Tensor, *, bias: Optional[torch.Tensor] = Non
          bcast_ptrs: Optional[list] = None, mc_ptr: int = 0, rms_in: Optional[torch.Tensor] = None,
          rms_eps: float = 0.0, sumsq_out: Optional[torch.Tensor] = None, trace: bool = False,
          splitk=True, ln_in=None, ln_colsum: Optional[torch.Tensor] = None,
-         rowsum_out: Optional[torch.Tensor] = None, rope=None, general_epilogue: bool = False) -> torch.Tensor:
+         rowsum_out: Optional[torch.Tensor] = None, rope=None) -> torch.Tensor:
     """out[M,Nout] = epi(a[M,K] @ w[N,K]^T); a/w may be row-strided views (last dim contiguous).
     `bn` forces the tile width (tests); 0 = library heuristic.
     `bcast_ptrs`: device pointers of peer buffers (same layout as `out`) that receive every output vector too
@@ -90,8 +90,7 @@ def gemm(a: torch.Tensor, w: torch.Tensor, *, bias: Optional[torch.Tensor] = Non
     `ln_in` = (row sums, row sums of squares) of `a`, both fp32 [M, parts], with `ln_colsum` (fp32 [N] = sum_k w[n,k]):
     LayerNorm folded into the GEMM (gamma folded into w, beta into bias; eps = `rms_eps`):
     rstd * (a w^T - mu * colsum) + bias.  `rowsum_out` (fp32 [M, N/32], together with `sumsq_out`): per-32-column sums of
-    the bf16 outputs, i.e. the statistics the NEXT folded LayerNorm needs.
-    `general_epilogue` (tests): run the kernel's general epilogue where the lean one (TMA stores) would be picked."""
+    the bf16 outputs, i.e. the statistics the NEXT folded LayerNorm needs."""
     _need_cuda(a, w, bias, residual, row_scale, out)
     _bf16(a, w, residual)
     assert a.dim() == 2 and w.dim() == 2 and a.stride(1) == 1 and w.stride(1) == 1, "gemm: 2-D, unit inner stride"
@@ -167,8 +166,6 @@ def gemm(a: torch.Tensor, w: torch.Tensor, *, bias: Optional[torch.Tensor] = Non
         args.mc_out = mc_ptr or None
     if trace:
         args.reserved2 = 777
-    if general_epilogue:
-        args.reserved4 = 1                          # test hook: the general epilogue instead of the lean (TMA-store) one
     forced = splitk is not True and splitk and int(splitk) > 1
     if forced or (splitk and _SPLITK_ENV):          # the workspace exists only when the split-K tail can actually run
         if forced:

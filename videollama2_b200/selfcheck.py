@@ -32,7 +32,7 @@ def fulldepth_check(model, fixture: str, pixels: torch.Tensor, input_ids: torch.
     `ok`.  `fixture` is a config name ("cfg2") or a path."""
     path = fixture if os.path.exists(fixture) else fixture_path(fixture)
     fx = torch.load(path, map_location="cpu")
-    rows, gold = fx["rows"], fx["g32"]
+    rows, gold = fx["rows"], {k: v.float() for k, v in fx["g32"].items()}   # stored as fp16
     dev = model.device
     inner = model.get_model()
     tower = inner.get_vision_tower()
