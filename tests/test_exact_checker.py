@@ -1,0 +1,95 @@
+"""Self-tests of the checks in test_kernels_exact_gpu.py, on the CPU: plant the faults a whole-tensor relL2 < 6e-3 lets
+through into a correct fp64 result and show that the element-wise checker rejects each of them, while it accepts the
+correctly rounded result.  Also checks on the CPU that the attention routing problems route (fp64 softmax is one-hot
+on the target)."""
+import math
+
+import pytest
+import torch
+
+from test_kernels_exact_gpu import (_routing_problem, attention_reference, check_elementwise, exact_softmax_scale,
+                                    gemm_acc_bound, gemm_bf16_bound, relerr)
+
+CPU = torch.device("cpu")
+
+
+def _bf16_randn(shape, scale, seed):
+    return (torch.randn(shape, generator=torch.Generator().manual_seed(seed)) * scale).to(torch.bfloat16)
+
+
+def test_checker_rejects_one_wrong_row():
+    """One row of an 1100-row GEMM output off by 10 %: relL2 3e-3, far under the 6e-3 bar."""
+    M, N, K = 1100, 1024, 328
+    a, w = _bf16_randn((M, K), 1.0, 1), _bf16_randn((N, K), 0.06, 2)
+    ref = a.double() @ w.double().t()
+    bound = gemm_bf16_bound(ref, gemm_acc_bound(a, w))
+    good = ref.float().to(torch.bfloat16)
+    assert check_elementwise(good, ref, bound, "correct") <= 1.0
+    bad = good.clone()
+    bad[517] = (bad[517].float() * 1.1).to(torch.bfloat16)
+    assert relerr(bad, ref) < 6e-3
+    with pytest.raises(AssertionError, match=r"row 517"):
+        check_elementwise(bad, ref, bound, "one row off")
+
+
+def test_checker_rejects_one_missing_k_block():
+    """One of 224 k-blocks (K = 14336, the decoder's down_proj depth) missing from one 128 x 64 tile of 256."""
+    M, N, K = 2048, 1024, 14336
+    a, w = _bf16_randn((M, K), 1.0, 3), _bf16_randn((N, K), K ** -0.5, 4)
+    ref = a.double() @ w.double().t()
+    bound = gemm_bf16_bound(ref, gemm_acc_bound(a, w))
+    good = ref.float().to(torch.bfloat16)
+    assert check_elementwise(good, ref, bound, "correct") <= 1.0
+    r0, c0, k0 = 5 * 128, 7 * 64, 100 * 64
+    faulty = ref.clone()
+    faulty[r0:r0 + 128, c0:c0 + 64] -= a[r0:r0 + 128, k0:k0 + 64].double() @ w[c0:c0 + 64, k0:k0 + 64].double().t()
+    bad = faulty.float().to(torch.bfloat16)
+    assert relerr(bad, ref) < 6e-3
+    with pytest.raises(AssertionError, match=r"in tile \(5, 7\)"):
+        check_elementwise(bad, ref, bound, "missing k-block", tile=(128, 64))
+
+
+def test_checker_rejects_one_leaked_masked_key():
+    """Causal attention (S = 512, 4 heads, D = 64, N(0, 1) logits) where row 40 of head 1 also sees key 41."""
+    S, H, D = 512, 4, 64
+    q, k, v = (_bf16_randn((H, S, D), 1.0, s) for s in (5, 6, 7))
+    scale = D ** -0.5
+    ref, bound = attention_reference(q, k, v, True, scale)
+    good = ref.float().to(torch.bfloat16)
+    assert check_elementwise(good, ref, bound, "correct", tile=(128, D)) <= 1.0
+    s = (q[1, 40].double() @ k[1, :42].double().t()) * scale
+    leaked = ref.clone()
+    leaked[1, 40] = torch.softmax(s, -1) @ v[1, :42].double()
+    bad = leaked.float().to(torch.bfloat16)
+    assert relerr(bad, ref) < 6e-3
+    with pytest.raises(AssertionError, match=r"row 40"):
+        check_elementwise(bad[1], ref[1], bound[1], "leaked key", tile=(128, D))
+
+
+@pytest.mark.parametrize("B,S,Hq,Hkv,D,causal", [(3, 257, 28, 4, 128, True), (3, 129, 4, 4, 40, False), (3, 45, 2, 2, 8, True),
+                                                 (1, 300, 4, 2, 72, True)])
+def test_routing_problem_is_one_hot(B, S, Hq, Hkv, D, causal):
+    """The logits the routing problems build give an fp64 softmax that is one-hot on the intended target, with the poison
+    keys (past the causal boundary, in the next batch's first rows) winning if they were visible."""
+    q, k, v, target = _routing_problem(B, S, Hq, Hkv, D, causal)
+    scale, sl2 = exact_softmax_scale()
+    assert sl2 == 0.125
+    G = Hq // Hkv
+    for b in range(B):
+        qf = q[b].transpose(0, 1)
+        kf = k[b].transpose(0, 1).repeat_interleave(G, 0)
+        s = (qf @ kf.transpose(1, 2)) * sl2                                 # log2 units
+        if causal:
+            s = s.masked_fill(torch.ones(S, S, dtype=torch.bool).triu(1), -math.inf)
+        top2 = s.topk(min(2, S), -1).values
+        assert torch.equal(s.argmax(-1), target[b].t())
+        if S > 1:
+            gap = top2[..., 0] - top2[..., 1]
+            rows_with_two = torch.isfinite(top2[..., 1])
+            assert bool((gap[rows_with_two] >= 40).all())
+        if b + 1 < B and S % 128:
+            # what a 2-D box past this batch's tail would read: the next batch's first rows beat every target
+            n_pad = min(S, -S % 128)
+            kn = k[b + 1, :n_pad].transpose(0, 1).repeat_interleave(G, 0)
+            leak = (qf @ kn.transpose(1, 2)) * sl2
+            assert bool((leak.amax(-1) > top2[..., 0]).all())
