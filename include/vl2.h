@@ -235,7 +235,8 @@ int vl2_row_stats(const void* x, float* sum_out, float* sumsq_out, int64_t rows,
 /* ------------------------------------------------------------------------------------------------------------
  * CLIP patch embedding front/back ends (HF:clip/modeling_clip.py:202-218).
  * vl2_patch_im2col: pixels bf16 [F,3,H,W] (NCHW) -> A bf16 [F*(H/P)*(W/P), Kpad], column = c*P*P + i*P + j, zero
- *   padded to Kpad (Kpad % 64 == 0) so the patch conv becomes vl2_gemm_bf16 against weight[1024, Kpad].  H / P and
+ *   padded to Kpad (Kpad % 64 == 0) so the patch conv becomes vl2_gemm_bf16 against weight[1024, Kpad].  P and W must
+ *   be even (pixel pairs are copied as one 4-byte word; CLIP and SigLIP use P = 14), else VL2_E_BADSHAPE.  H / P and
  *   W / P round down like the strided conv does (SigLIP@384, P = 14: 27 x 27 patches, the last 6 pixels are unused).
  * vl2_clip_embed_finish: tok[f, 0] = cls + pos[0]; tok[f, 1+p] = patch[f*np+p] + pos[1+p]; then pre_layrnorm.
  * ---------------------------------------------------------------------------------------------------------- */

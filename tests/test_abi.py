@@ -40,8 +40,30 @@ def test_struct_layouts_match_header():
     assert ctypes.sizeof(AttnArgs) == 4 * 8 + 4 * 8 + 8 * 4
 
 
+BADSHAPE, BADALIGN = -1, -3
+A16, MIS = 4096, 4104          # fake device addresses: 16-byte aligned, and 8 bytes off (never dereferenced)
+ROW_ARGUMENT_CASES = [
+    # odd P: a pixel pair at an odd element offset would be loaded as one misaligned 4-byte word
+    ("vl2_patch_im2col", (A16, A16, 1, 15, 16, 15, 680, None), BADSHAPE),
+    ("vl2_patch_im2col", (A16, A16, 1, 14, 14, 7, 152, None), BADSHAPE),
+    ("vl2_patch_im2col", (A16 + 2, A16, 1, 14, 14, 14, 592, None), BADALIGN),
+    # 16-byte vector accesses: every pointer they touch is checked
+    ("vl2_se_scale", (MIS, A16, 1, 4, 64, None), BADALIGN),
+    ("vl2_se_scale", (A16, MIS, 1, 4, 64, None), BADALIGN),
+    ("vl2_clip_embed_finish", (A16, A16, A16, MIS, A16, A16, 1, 4, 64, 1e-5, None), BADALIGN),
+    ("vl2_clip_embed_finish", (A16, A16, A16, A16, MIS, A16, 1, 4, 64, 1e-5, None), BADALIGN),
+    ("vl2_embed_splice", (A16, A16, 2, MIS, 100, A16, 64, None), BADALIGN),
+    ("vl2_embed_splice", (A16, A16, 2, A16, 100, MIS, 64, None), BADALIGN),
+    ("vl2_conv3d_im2col", (MIS, A16, 2, 4, 4, 64, 1, 2, 3, 3, None), BADALIGN),
+    ("vl2_conv3d_im2col", (A16, MIS, 2, 4, 4, 64, 1, 2, 3, 3, None), BADALIGN),
+    ("vl2_decode_rope_append", (MIS, A16, 768, A16, 4, 1, 128, A16, 1, None), BADALIGN),
+    ("vl2_decode_rope_append", (A16, MIS, 768, A16, 4, 1, 128, A16, 1, None), BADALIGN),
+]
+
+
 def test_argument_validation_without_gpu(lib):
-    """Shape/alignment checks run before any CUDA call, so they are testable on CPU."""
+    """Shape/alignment checks run before any CUDA call, so they are testable on CPU.  Odd patch sizes and misaligned
+    pointers are refused with VL2_E_BADSHAPE / VL2_E_BADALIGN (the kernels would fault on a misaligned vector access)."""
     from videollama2_b200._lib import GemmArgs
     a = GemmArgs(A=16, W=16, C=16, lda=8, ldw=8, ldc=8, ldr=0, M=4, N=8, K=12, act=0, out_f32=0)
     assert lib.vl2_gemm_bf16(ctypes.byref(a), None) == -1 and b"multiples of 8" in lib.vl2_last_error()
@@ -49,6 +71,8 @@ def test_argument_validation_without_gpu(lib):
     assert lib.vl2_gemm_bf16(ctypes.byref(a), None) == -3
     a = GemmArgs(A=16, W=16, C=16, lda=8, ldw=8, ldc=8, ldr=0, M=4, N=8, K=8, act=9, out_f32=0)
     assert lib.vl2_gemm_bf16(ctypes.byref(a), None) == -6
+    for name, args, code in ROW_ARGUMENT_CASES:
+        assert getattr(lib, name)(*args) == code, (name, args, lib.vl2_last_error())
 
 
 def test_ops_refuse_cpu_tensors():

@@ -1,14 +1,17 @@
-"""Self-tests of the checks in test_kernels_exact_gpu.py, on the CPU: plant the faults a whole-tensor relL2 < 6e-3 lets
-through into a correct fp64 result and show that the element-wise checker rejects each of them, while it accepts the
-correctly rounded result.  Also checks on the CPU that the attention routing problems route (fp64 softmax is one-hot
-on the target)."""
+"""Self-tests of the checks in test_kernels_exact_gpu.py and test_rowops_decode_exact_gpu.py, on the CPU: plant the
+faults a whole-tensor relL2 < 6e-3 lets through into a correct fp64 result and show that the element-wise checker
+rejects each of them, while it accepts the correctly rounded result.  Also checks on the CPU that the attention routing
+problems route (fp64 softmax is one-hot on the target) and that the RoPE table matcher tells rounding noise from a
+wrong table."""
 import math
 
 import pytest
 import torch
 
-from test_kernels_exact_gpu import (_routing_problem, attention_reference, check_elementwise, exact_softmax_scale,
-                                    gemm_acc_bound, gemm_bf16_bound, relerr)
+from test_kernels_exact_gpu import (_ln_rows_bound, _routing_problem, attention_reference, check_elementwise,
+                                    exact_softmax_scale, gemm_acc_bound, gemm_bf16_bound, relerr)
+from test_rowops_decode_exact_gpu import (ROPE_POSITIONS, ROPE_THETA, rope_angles_fp32, rope_table_mismatches,
+                                          rope_table_parts)
 
 CPU = torch.device("cpu")
 
@@ -93,3 +96,64 @@ def test_routing_problem_is_one_hot(B, S, Hq, Hkv, D, causal):
             kn = k[b + 1, :n_pad].transpose(0, 1).repeat_interleave(G, 0)
             leak = (qf @ kn.transpose(1, 2)) * sl2
             assert bool((leak.amax(-1) > top2[..., 0]).all())
+
+
+def test_checker_rejects_one_layernorm_row_one_percent_off():
+    """LayerNorm of 1521 rows x 1024 with one row 1 % off: relL2 < 4e-3 (the bar of the relL2 LayerNorm tests) passes
+    it, the _ln_rows_bound check does not."""
+    R, C = 1521, 1024
+    x = _bf16_randn((R, C), 1.0, 8).double()
+    gamma = (_bf16_randn((C,), 0.1, 9).float() + 1).to(torch.bfloat16).double()
+    beta = _bf16_randn((C,), 0.5, 10).double()
+    ref, err = _ln_rows_bound(x, torch.zeros_like(x), gamma, beta)
+    bound = gemm_bf16_bound(ref, err)
+    good = ref.float().to(torch.bfloat16)
+    assert check_elementwise(good, ref, bound, "correct") <= 1.0
+    bad = good.clone()
+    bad[700] = (bad[700].float() * 1.01).to(torch.bfloat16)
+    assert relerr(bad, ref) < 4e-3
+    with pytest.raises(AssertionError, match=r"row 700"):
+        check_elementwise(bad, ref, bound, "one row 1 % off")
+
+
+def _rope_fp64_table(ang32):
+    """bf16 cos / sin of the fp32 angles rounded from fp64: the correctly rounded table."""
+    a = ang32.double()
+    return a.cos().float().to(torch.bfloat16), a.sin().float().to(torch.bfloat16)
+
+
+@pytest.mark.parametrize("D", [128, 64])
+def test_rope_matcher_accepts_host_table(D):
+    """ops.rope_table (fp32 cos / sin of torch) against the correctly rounded table over 32768 positions: the few
+    differences are one-ulp roundings next to a midpoint, which the matcher accepts."""
+    from videollama2_b200 import ops
+    ang = rope_angles_fp32(ROPE_POSITIONS, D)
+    tc, ts = rope_table_parts(ops.rope_table(ROPE_POSITIONS, D, ROPE_THETA, "cpu"))
+    fc, fs = _rope_fp64_table(ang)
+    n = rope_table_mismatches(tc, ts, fc, fs, ang)
+    assert n <= 64, n
+    assert rope_table_mismatches(tc, ts, tc, ts, ang) == 0
+
+
+def test_rope_matcher_rejects_off_by_one_position():
+    """The table of position p + 1 used for position p."""
+    from videollama2_b200 import ops
+    D = 128
+    tc, ts = rope_table_parts(ops.rope_table(ROPE_POSITIONS + 1, D, ROPE_THETA, "cpu"))
+    ang = rope_angles_fp32(ROPE_POSITIONS, D)
+    with pytest.raises(AssertionError, match="differs at position"):
+        rope_table_mismatches(tc[1:], ts[1:], tc[:-1], ts[:-1], ang)
+
+
+def test_rope_matcher_rejects_fp32_range_reduction():
+    """cos / sin after reducing the angle modulo 2 pi in fp32 arithmetic (the reduction loses up to |angle| 2^-24 of
+    absolute accuracy, up to 2^-9 at position 32767): wrong far from any rounding midpoint."""
+    from videollama2_b200 import ops
+    D = 128
+    ang = rope_angles_fp32(ROPE_POSITIONS, D)
+    two_pi = torch.tensor(2 * math.pi, dtype=torch.float32)
+    red = ang - torch.round(ang / two_pi) * two_pi
+    rc, rs = _rope_fp64_table(red)
+    tc, ts = rope_table_parts(ops.rope_table(ROPE_POSITIONS, D, ROPE_THETA, "cpu"))
+    with pytest.raises(AssertionError, match="differs at position"):
+        rope_table_mismatches(rc, rs, tc, ts, ang)

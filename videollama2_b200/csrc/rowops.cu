@@ -300,17 +300,7 @@ __global__ void patch_im2col_kernel(const __nv_bfloat16* __restrict__ px, __nv_b
       const int pw = (int)(row % gw), ph = (int)((row / gw) % gh), f = (int)(row / ((int64_t)gw * gh));
       const int c = col / (P * P), r = col % (P * P), i = r / P, j = r % P;
       const __nv_bfloat16* s = px + (((int64_t)f * 3 + c) * H + (ph * P + i)) * W + pw * P + j;
-      if (j + 1 < P) {
-        out = *reinterpret_cast<const uint32_t*>(s);  // P even, j even => 4-byte aligned, same image row
-      } else {
-        out = (uint32_t)__bfloat16_as_ushort(s[0]);
-        // odd P: the pair straddles kernel rows / channels
-        const int col1 = col + 1;
-        if (col1 < K) {
-          const int c1 = col1 / (P * P), r1 = col1 % (P * P), i1 = r1 / P, j1 = r1 % P;
-          out |= (uint32_t)__bfloat16_as_ushort(px[(((int64_t)f * 3 + c1) * H + (ph * P + i1)) * W + pw * P + j1]) << 16;
-        }
-      }
+      out = *reinterpret_cast<const uint32_t*>(s);  // P, W and j even => 4-byte aligned, (j, j+1) in one image row
     }
     *reinterpret_cast<uint32_t*>(A + row * Kpad + col) = out;
   }
@@ -844,8 +834,10 @@ extern "C" int vl2_row_stats(const void* x, float* sum_out, float* sumsq_out, in
 
 extern "C" int vl2_patch_im2col(const void* pixels, void* A, int F, int H, int W, int P, int Kpad, void* stream) {
   VL2_REQUIRE(F > 0 && P > 0 && H >= P && W >= P, VL2_E_BADSHAPE, "vl2_patch_im2col: H,W must be at least P");
-  VL2_REQUIRE(Kpad % 8 == 0 && Kpad >= 3 * P * P && W % 2 == 0, VL2_E_BADSHAPE,
-              "vl2_patch_im2col: Kpad %% 8 == 0, Kpad >= 3*P*P and even W required");
+  VL2_REQUIRE(Kpad % 8 == 0 && Kpad >= 3 * P * P && W % 2 == 0 && P % 2 == 0, VL2_E_BADSHAPE,
+              "vl2_patch_im2col: Kpad %% 8 == 0, Kpad >= 3*P*P, even W and even P required (P=%d)", P);
+  VL2_REQUIRE((reinterpret_cast<uintptr_t>(pixels) & 3) == 0 && (reinterpret_cast<uintptr_t>(A) & 3) == 0, VL2_E_BADALIGN,
+              "vl2_patch_im2col: pixels and A must be 4-byte aligned (pixel pairs are copied as one word)");
   const int64_t total = (int64_t)F * (H / P) * (W / P) * (Kpad / 2);
   launch_kernel(patch_im2col_kernel, dim3(grid_for(total, 256)), dim3(256), 0, (cudaStream_t)stream, 1, (const bf16*)pixels, (bf16*)A, F, H, W, P,
                                                                              Kpad);
@@ -856,7 +848,8 @@ extern "C" int vl2_patch_im2col(const void* pixels, void* A, int F, int H, int W
 extern "C" int vl2_clip_embed_finish(const void* patch, const void* cls, const void* pos, const void* gamma,
                                      const void* beta, void* tok, int F, int np, int C, float eps, void* stream) {
   VL2_REQUIRE(F > 0 && np > 0 && C % 8 == 0 && C <= 512 * 8 * kMaxVec, VL2_E_BADSHAPE, "vl2_clip_embed_finish: bad shape");
-  VL2_REQUIRE(aligned16(patch) && aligned16(cls) && aligned16(pos) && aligned16(tok), VL2_E_BADALIGN,
+  VL2_REQUIRE(aligned16(patch) && aligned16(cls) && aligned16(pos) && aligned16(gamma) && aligned16(beta) && aligned16(tok),
+              VL2_E_BADALIGN,
               "vl2_clip_embed_finish: 16-byte alignment");
   launch_kernel(clip_embed_finish_kernel, dim3((unsigned)(F * (np + 1))), dim3(row_threads(C)), 0, (cudaStream_t)stream, 1, 
       (const bf16*)patch, (const bf16*)cls, (const bf16*)pos, (const bf16*)gamma, (const bf16*)beta, (bf16*)tok, np, C,
@@ -893,6 +886,7 @@ extern "C" int vl2_dwconv3x3_ln_silu(const void* x, const void* w9c, const void*
 
 extern "C" int vl2_se_scale(void* y, const float* s, int F, int HW, int C, void* stream) {
   VL2_REQUIRE(F > 0 && HW > 0 && C % 8 == 0, VL2_E_BADSHAPE, "vl2_se_scale: bad shape");
+  VL2_REQUIRE(aligned16(y) && aligned16(s), VL2_E_BADALIGN, "vl2_se_scale: 16-byte alignment");
   const int64_t total = (int64_t)F * HW * (C / 8);
   launch_kernel(se_scale_kernel, dim3(grid_for(total, 256)), dim3(256), 0, (cudaStream_t)stream, 1, (bf16*)y, s, HW, C, total);
   VL2_CHECK_LAUNCH("se_scale_kernel");
@@ -903,6 +897,7 @@ extern "C" int vl2_conv3d_im2col(const void* x, void* A, int T, int H, int W, in
                                  void* stream) {
   VL2_REQUIRE(T > 0 && H > 0 && W > 0 && C % 8 == 0 && To > 0 && Ho > 0 && Wo > 0 && (pad == 0 || pad == 1),
               VL2_E_BADSHAPE, "vl2_conv3d_im2col: bad shape");
+  VL2_REQUIRE(aligned16(x) && aligned16(A), VL2_E_BADALIGN, "vl2_conv3d_im2col: 16-byte alignment");
   const int64_t total = (int64_t)To * Ho * Wo * 8 * (C / 8);
   launch_kernel(conv3d_im2col_kernel, dim3(grid_for(total, 256)), dim3(256), 0, (cudaStream_t)stream, 1, (const bf16*)x, (bf16*)A, T, H, W, C, pad,
                                                                               To, Ho, Wo);
@@ -926,6 +921,7 @@ extern "C" int vl2_rope_inplace(void* qkv, int64_t ld, int S, int Hq, int Hkv, i
 extern "C" int vl2_embed_splice(const int64_t* ids, const int32_t* dst_row, int n, const void* table, int64_t vocab,
                                 void* out, int H, void* stream) {
   VL2_REQUIRE(n > 0 && H % 8 == 0, VL2_E_BADSHAPE, "vl2_embed_splice: bad shape");
+  VL2_REQUIRE(aligned16(table) && aligned16(out), VL2_E_BADALIGN, "vl2_embed_splice: 16-byte alignment");
   launch_kernel(embed_splice_kernel, dim3(n), dim3(128), 0, (cudaStream_t)stream, 1, ids, dst_row, (const bf16*)table, vocab, (bf16*)out, H);
   VL2_CHECK_LAUNCH("embed_splice_kernel");
   return VL2_OK;
@@ -956,6 +952,7 @@ extern "C" int vl2_decode_rope_append(void* qkv_row, void* cache, int64_t cache_
                                       int D, const float* inv_freq, int interleaved, void* stream) {
   VL2_REQUIRE(qkv_row && cache && pos_dev && inv_freq && D % 16 == 0 && cache_ld % 8 == 0, VL2_E_BADSHAPE,
               "vl2_decode_rope_append: bad arguments");
+  VL2_REQUIRE(aligned16(qkv_row) && aligned16(cache), VL2_E_BADALIGN, "vl2_decode_rope_append: 16-byte alignment");
   const int width = (Hq + 2 * Hkv) * D;
   int threads = (Hq + Hkv) * (D / 16);
   threads = threads > 512 ? 512 : ((threads + 31) / 32 * 32);
