@@ -144,12 +144,14 @@ typedef struct vl2_gemm_args {
   int32_t rope_cols, rope_D, rope_pos0, reserved5;
 } vl2_gemm_args;
 int vl2_gemm_bf16(const vl2_gemm_args* args, void* stream);
-/* Debug aid: with args->reserved2 == 777 CTA 0 records clock64() at its tile boundaries: out[0] = tiles traced (<= 7), and
- * for tile t at out[8t+1..8t+6]: MMA role waits for the accumulator stage / starts issuing / issued its last commit;
- * epilogue warp starts the tile / sees the accumulator complete / stored its last span; out[64+8t .. 64+8t+5]: phases of that
- * warp's first 64-column span (start, residual staged, accumulator chunk loaded, first / second half computed, stored).
- * host_out128: 128 values.  Synchronises the device. */
+/* Debug aid: with args->reserved2 == 777 the first consumer thread of CTA 0 records clock64() at its tile boundaries:
+ * out[0] = tiles traced (<= 7), and for tile t: out[8t+4] = starts the tile's k-loop, out[8t+5] = accumulator complete,
+ * out[8t+6] = its part of the tile stored.  host_out128: 128 values.  Synchronises the device. */
 int vl2_debug_gemm_trace(long long* host_out128);
+/* How many CTAs (pair = 0) or two-CTA clusters (pair = 1) of the GEMM kernel with tile width bn the current device runs at
+ * once (occupancy API at the kernel's shared-memory size).  The persistent grid of vl2_gemm_bf16 is min(tiles, SMs) CTAs or
+ * min(tiles, SMs / 2) pairs, which must not exceed it. */
+int vl2_gemm_coresident(int bn, int pair, int32_t* out);
 /* Planning only, no device work: out6 = {tile width BN, 1 if the 256-row two-CTA tile is used, number of tiles,
  * CTAs (or CTA pairs) the persistent grid runs, rounds = ceil(tiles / that), SM count assumed (132, an H100 SXM, without a device)}. */
 int vl2_gemm_plan(int M, int N, int K, int with_splitk_ws, int32_t* out6);

@@ -12,7 +12,7 @@ LIB_PATH_F16 = os.environ.get("VL2_LIBVL2_F16") or os.path.join(_HERE, "libvl2_f
 # Every symbol include/vl2.h declares (tests/test_abi.py checks the header against this list and the .so).
 SYMBOLS = [
     "vl2_version", "vl2_storage_dtype", "vl2_last_error", "vl2_launch_count",
-    "vl2_gemm_bf16", "vl2_gemm_skinny", "vl2_attention", "vl2_attention_decode", "vl2_debug_attn_trace", "vl2_debug_gemm_trace", "vl2_gemm_plan",
+    "vl2_gemm_bf16", "vl2_gemm_skinny", "vl2_attention", "vl2_attention_decode", "vl2_debug_attn_trace", "vl2_debug_gemm_trace", "vl2_gemm_plan", "vl2_gemm_coresident",
     "vl2_decode_rope_append", "vl2_attention_decode_dyn", "vl2_gemv_bf16", "vl2_attention_decode_workspace", "vl2_set_pdl", "vl2_l2_prefetch", "vl2_preprocess_frames", "vl2_preprocess_workspace",
     "vl2_layernorm", "vl2_rmsnorm", "vl2_row_sumsq", "vl2_row_stats",
     "vl2_patch_im2col", "vl2_clip_embed_finish",

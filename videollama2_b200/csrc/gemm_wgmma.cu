@@ -135,6 +135,17 @@ __device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned* p) {
   asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
   return v;
 }
+// A consumer warp hands a ring slot back to the producer(s).  A pair releases it in both CTAs, since the peer's multicast
+// also writes into it.  No memory fence is needed: the slot holds only wgmma operands, whose (async-proxy) reads are
+// complete once wgmma.wait_group has returned, and the next write into the slot is a TMA load that the producer issues only
+// after its mbarrier wait has observed this arrival.  So the arrival publishes no data and needs no release at cluster
+// scope; mbar_arrive_cluster (release.cluster) would put a GPU-scope MEMBAR in every consumer warp's k-loop.
+template <bool PAIR>
+__device__ __forceinline__ void release_slot(uint64_t* empty_bar, uint32_t rank) {
+  mbar_arrive(empty_bar);
+  if (PAIR) mbar_arrive_peer(empty_bar, rank ^ 1u);
+}
+
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory"); }
 
 // sum the producer's per-32-column partials of one row in a fixed order (deterministic: no atomics anywhere)
@@ -190,12 +201,49 @@ __device__ __forceinline__ void gemm_epilogue(float (&acc)[BN / 2], const GemmPa
   }
   const __nv_bfloat16* res = reinterpret_cast<const __nv_bfloat16*>(p.residual);
   __nv_bfloat16* cb = reinterpret_cast<__nv_bfloat16*>(p.C);
-#pragma unroll
-  for (int s = 0; s < BN / 32; ++s) {      // 32-column slots
+  // 32-column slots, one per iteration and NOT unrolled.  A slot's code carries every epilogue feature, about 340
+  // instructions per column pair.  Unrolled over all BN / 32 slots it made a ~400 KB kernel, far more than the SM's
+  // instruction caches hold, and the epilogue of a 128 x 256 tile took ~200 k cycles in the kernel's trace; rolled here
+  // and over the 8-column groups below, the kernel is ~3.5 k instructions and the same epilogue takes ~50 k.  Registers
+  // cannot be indexed at run time, so each iteration first selects its slot's 16 accumulators into v[] with compile-time
+  // indices.
+#pragma unroll 1
+  for (int s = 0; s < BN / 32; ++s) {
     if (n0 + 32 * s >= p.N) break;         // uniform over the warpgroup
-    float ssq[2] = {0.f, 0.f}, ssum[2] = {0.f, 0.f};
+    float v[16];
 #pragma unroll
-    for (int jj = 0; jj < 4; ++jj) {
+    for (int k = 0; k < BN / 32; ++k) {
+      if (k == s) {
+#pragma unroll
+        for (int i = 0; i < 16; ++i) v[i] = acc[16 * k + i];
+      }
+    }
+    // the slot's residuals in one batch of loads: one L2 round trip per slot instead of one per column pair.  A residual
+    // that aliases the output is read at this thread's own output positions only, before the thread writes them.
+    uint32_t rv[4][2] = {};
+    if (res != nullptr) {
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        const int c = n0 + 8 * (4 * s + jj) + 2 * t;
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          if (n0 + 8 * (4 * s + jj) < p.N && ok[h]) rv[jj][h] = *reinterpret_cast<const uint32_t*>(res + (int64_t)rows[h] * p.ldr + c);
+      }
+    }
+    float ssq[2] = {0.f, 0.f}, ssum[2] = {0.f, 0.f};
+#pragma unroll 1
+    for (int jj = 0; jj < 4; ++jj) {   // 8-column groups, not unrolled either: the loop body is two column pairs
+      float vj[4] = {v[0], v[1], v[2], v[3]};
+      uint32_t rj[2] = {rv[0][0], rv[0][1]};
+#pragma unroll
+      for (int k = 1; k < 4; ++k) {
+        if (k == jj) {
+#pragma unroll
+          for (int i = 0; i < 4; ++i) vj[i] = v[4 * k + i];
+          rj[0] = rv[k][0];
+          rj[1] = rv[k][1];
+        }
+      }
       const int j = 4 * s + jj;
       const int c = n0 + 8 * j + 2 * t;    // this thread's column pair
       const bool col_ok = n0 + 8 * j < p.N;   // N % 8 == 0: the whole 8-column group is in or out
@@ -204,7 +252,7 @@ __device__ __forceinline__ void gemm_epilogue(float (&acc)[BN / 2], const GemmPa
       if (col_ok && ln) cs = __ldg(reinterpret_cast<const float2*>(p.ln_colsum + c));
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
+        float x0 = vj[2 * h], x1 = vj[2 * h + 1];
         if (ln) { x0 = fmaf(-mu[h], cs.x, x0); x1 = fmaf(-mu[h], cs.y, x1); }
         x0 = x0 * rs[h] + bq.x;
         x1 = x1 * rs[h] + bq.y;
@@ -228,9 +276,8 @@ __device__ __forceinline__ void gemm_epilogue(float (&acc)[BN / 2], const GemmPa
           x1 = b * co + a * sn;
         }
         if (res != nullptr && st_ok) {
-          const uint32_t r = *reinterpret_cast<const uint32_t*>(res + (int64_t)rows[h] * p.ldr + c);
-          x0 += bf16_lo(r);
-          x1 += bf16_hi(r);
+          x0 += bf16_lo(rj[h]);
+          x1 += bf16_hi(rj[h]);
         }
         if (p.out_f32) {
           if (st_ok) *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.C) + (int64_t)rows[h] * p.ldc + c) = make_float2(x0, x1);
@@ -371,19 +418,13 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
         for (int k = 0; k < BK / 16; ++k) Wgmma<BN, 0>::ss(acc, da + 2 * k, db + 2 * k, (kb != w.kb0 || k != 0) ? 1u : 0u);
         wgmma_commit();
         wgmma_wait<1>();            // the previous k-block's MMAs are complete: its ring slot can be refilled
-        if (prev >= 0 && lane == 0) {
-          if (PAIR) { mbar_arrive_cluster(&empty_bar[prev], 0); mbar_arrive_cluster(&empty_bar[prev], 1); }
-          else mbar_arrive(&empty_bar[prev]);
-        }
+        if (prev >= 0 && lane == 0) release_slot<PAIR>(&empty_bar[prev], rank);
         prev = stage;
         if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
       }
       wgmma_wait<0>();
       wgmma_keep(acc);
-      if (lane == 0) {
-        if (PAIR) { mbar_arrive_cluster(&empty_bar[prev], 0); mbar_arrive_cluster(&empty_bar[prev], 1); }
-        else mbar_arrive(&empty_bar[prev]);
-      }
+      if (lane == 0) release_slot<PAIR>(&empty_bar[prev], rank);
       if (tr && it < 7) g_gemm_trace[8 * it + 5] = clock64();
       const int slot = (tile - p.split_first) * (p.split_s - 1);   // workspace slot of a split tile's slices
       // partials layout per CTA: [accumulator quad][consumer thread][4 floats] (every warp access is one 512-byte piece)
@@ -452,6 +493,35 @@ static double kb_cycles(int bn, bool pair) {
   return c > lat ? c : lat;
 }
 
+
+// How many persistent units (CTAs, or CTA pairs) of this instantiation the current device can run at once, or a negative
+// VL2_E_* code.  A pair needs two free SMs of one GPC, so fewer than sm_count() / 2 pairs may fit; on an H100 SXM
+// (132 SMs) all 66 pairs of every width fit, which the persistent grid of launch_gemm assumes.
+template <int BN, bool PAIR>
+static int coresident_units() {
+  using Cfg = GemmCfg<BN, PAIR>;
+  VL2_SMEM_OPT_IN((gemm_bf16_wgmma_kernel<BN, PAIR>), Cfg::kSmemBytes);
+  int n = 0;
+  if (PAIR) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(sm_count() & ~1);
+    cfg.blockDim = dim3(kGemmThreads);
+    cfg.dynamicSmemBytes = Cfg::kSmemBytes;
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = 2;
+    attr.val.clusterDim.y = 1;
+    attr.val.clusterDim.z = 1;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
+    VL2_CHECK_CUDA(cudaOccupancyMaxActiveClusters(&n, gemm_bf16_wgmma_kernel<BN, PAIR>, &cfg));
+  } else {
+    VL2_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, gemm_bf16_wgmma_kernel<BN, PAIR>, kGemmThreads,
+                                                                 Cfg::kSmemBytes));
+    n *= sm_count();
+  }
+  return n;
+}
 
 template <int BN, bool PAIR>
 static int launch_gemm(const vl2_gemm_args* a, cudaStream_t stream) {
@@ -623,6 +693,37 @@ extern "C" int vl2_gemm_plan(int M, int N, int K, int with_splitk_ws, int32_t* o
   out6[3] = slots;
   out6[4] = (tiles + slots - 1) / slots;   // rounds of the persistent loop
   out6[5] = sms;
+  return VL2_OK;
+}
+
+// How many CTAs (pair = 0) or CTA pairs (pair = 1) of the BN-wide GEMM kernel the current device runs at once, from the
+// occupancy API at the kernel's shared-memory size.
+extern "C" int vl2_gemm_coresident(int bn, int pair, int32_t* out) {
+  using namespace vl2;
+  VL2_REQUIRE(out != nullptr && bn >= 64 && bn <= 256 && bn % 32 == 0 && (pair == 0 || bn >= 128), VL2_E_BADSHAPE,
+              "vl2_gemm_coresident: bad arguments (bn %d, pair %d)", bn, pair);
+  int n;
+  if (pair) {
+    switch (bn) {
+      case 256: n = coresident_units<256, true>(); break;
+      case 224: n = coresident_units<224, true>(); break;
+      case 192: n = coresident_units<192, true>(); break;
+      case 160: n = coresident_units<160, true>(); break;
+      default: n = coresident_units<128, true>(); break;
+    }
+  } else {
+    switch (bn) {
+      case 256: n = coresident_units<256, false>(); break;
+      case 224: n = coresident_units<224, false>(); break;
+      case 192: n = coresident_units<192, false>(); break;
+      case 160: n = coresident_units<160, false>(); break;
+      case 128: n = coresident_units<128, false>(); break;
+      case 96: n = coresident_units<96, false>(); break;
+      default: n = coresident_units<64, false>(); break;
+    }
+  }
+  if (n < 0) return n;
+  *out = n;
   return VL2_OK;
 }
 

@@ -253,12 +253,24 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-// arrive on the barrier at the same smem offset in CTA `rank` of the cluster
+// arrive on the barrier at the same smem offset in CTA `rank` of the cluster, releasing this thread's prior writes at
+// cluster scope: for an arrival that publishes data written through DSMEM.  ptxas puts a GPU-scope MEMBAR in front of it.
 __device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar_local, uint32_t rank) {
   asm volatile(
       "{\n\t.reg .b32 ra;\n\t"
       "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
       "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}"
+      ::"r"(smem_u32(bar_local)), "r"(rank)
+      : "memory");
+}
+// The same arrival without the cluster-scope release (default semantics: release at CTA scope), which compiles to a bare
+// SYNCS.ARRIVE with no memory barrier.  Enough for a signal that publishes no data of its own, e.g. "I have finished
+// reading this ring slot" when the reads were async-proxy (wgmma) reads already complete at wgmma.wait_group.
+__device__ __forceinline__ void mbar_arrive_peer(uint64_t* bar_local, uint32_t rank) {
+  asm volatile(
+      "{\n\t.reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}"
       ::"r"(smem_u32(bar_local)), "r"(rank)
       : "memory");
 }
