@@ -159,3 +159,49 @@ def test_gemm_plan_for_the_path_shapes(lib):
     assert small["pair"] == 0 and small["bn"] <= 128 and small["rounds"] == 1
     out = (ctypes.c_int32 * 6)()
     assert lib.vl2_gemm_plan(0, 8, 8, 0, out) < 0
+
+
+def test_ops_validate_out_and_inv_freq_before_launch(monkeypatch):
+    """attention / attention_decode refuse an `out` of another type than the operands (a bf16 or fp32 buffer would be
+    filled with fp16 bit patterns) or of the wrong shape, and decode_rope_append an inv_freq that is not fp32 [D / 2],
+    before anything is launched: the device check and the library are replaced by stand-ins, and a launch fails."""
+    import torch
+    from videollama2_b200 import ops
+
+    class Launched(Exception):
+        pass
+
+    def no_launch(t):
+        raise Launched("a kernel was launched")
+
+    monkeypatch.setattr(ops, "_need_cuda", lambda *ts: None)
+    monkeypatch.setattr(ops, "_L", no_launch)
+    monkeypatch.setattr(ops, "_stream", lambda: 0)
+    monkeypatch.setattr(ops, "decode_workspace", lambda *a: torch.zeros(16))
+    B, S, Hq, Hkv, D = 1, 8, 4, 2, 64
+    h = torch.float16
+    q, k, v = torch.zeros(B * S, Hq * D, dtype=h), torch.zeros(B * S, Hkv * D, dtype=h), torch.zeros(B * S, Hkv * D, dtype=h)
+    kw = dict(B=B, S=S, Hq=Hq, Hkv=Hkv, D=D, causal=True, scale=0.125)
+    for bad in (torch.bfloat16, torch.float32):
+        with pytest.raises(TypeError):
+            ops.attention(q, k, v, out=torch.zeros(B * S, Hq * D, dtype=bad), **kw)
+    with pytest.raises(AssertionError):
+        ops.attention(q, k, v, out=torch.zeros(B * S, Hq * D - 8, dtype=h), **kw)
+    with pytest.raises(Launched):
+        ops.attention(q, k, v, out=torch.zeros(B * S, Hq * D, dtype=h), **kw)
+    qd, cache = torch.zeros(Hq * D, dtype=h), torch.zeros(16, (Hq + 2 * Hkv) * D, dtype=h)
+    kc, vc = cache[:, Hq * D:(Hq + Hkv) * D], cache[:, (Hq + Hkv) * D:]
+    kw = dict(n_pos=16, Hq=Hq, Hkv=Hkv, D=D, scale=0.125)
+    for bad in (torch.bfloat16, torch.float32):
+        with pytest.raises(TypeError):
+            ops.attention_decode(qd, kc, vc, out=torch.zeros(1, Hq * D, dtype=bad), **kw)
+    with pytest.raises(AssertionError):
+        ops.attention_decode(qd, kc, vc, out=torch.zeros(1, Hq * D // 2, dtype=h), **kw)
+    with pytest.raises(Launched):
+        ops.attention_decode(qd, kc, vc, out=torch.zeros(1, Hq * D, dtype=h), **kw)
+    row, pos = torch.zeros(1, (Hq + 2 * Hkv) * D, dtype=h), torch.zeros(1, dtype=torch.int32)
+    for inv in (torch.zeros(D // 2, dtype=torch.float64), torch.zeros(D // 2, dtype=h), torch.zeros(D, dtype=torch.float32)):
+        with pytest.raises(AssertionError):
+            ops.decode_rope_append(row, cache, pos, Hq, Hkv, D, inv)
+    with pytest.raises(Launched):
+        ops.decode_rope_append(row, cache, pos, Hq, Hkv, D, torch.zeros(D // 2, dtype=torch.float32))

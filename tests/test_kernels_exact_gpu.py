@@ -1,26 +1,43 @@
 """The tensor-core kernels (wgmma GEMM with its pair tiles, split-K and Conv3d front end; FlashAttention; split-KV decode
 attention; fused patch embedding) checked bit for bit where the right answer is known exactly, and element by element
-against a bound derived from the kernel's own roundings where it is not.
+against a bound derived from the kernel's own roundings where it is not.  Every test runs on both builds of the library,
+bf16 storage (libvl2.so) and IEEE fp16 storage (libvl2_f16.so, the same sources with other conversion instructions and
+wgmma / TMA types): the `dt` parameter; the bf16 cases keep their original ids, the fp16 ones are [fp16-...] (a test
+without other parameters has an fp16 sibling named ..._fp16).
 
-A whole-tensor relL2 dilutes a fault confined to one row, one tile or one k-block below the bf16 noise floor; the checks
-here do not: every element is compared on its own (see test_exact_checker.py for the faults each check rejects).
+A whole-tensor relL2 dilutes a fault confined to one row, one tile or one k-block below the 16-bit noise floor; the
+checks here do not: every element is compared on its own (see test_exact_checker.py for the faults each check rejects).
 
 Exact sections
   * GEMM: small-integer operands make every product and partial sum an integer far below 2^24, so the fp32 accumulation
-    is exact in any order and the output equals the fp64 product (fp32) or its round-to-nearest-even (bf16).
+    is exact in any order and the output equals the fp64 product (fp32) or its round-to-nearest-even (bf16 / fp16).  In
+    fp16 integers above 2048 round too; that is still one rounding of an fp32-exact value (to_storage_exact).  Nothing
+    reaches 65504 by construction in the random tests only because the random sums stay small, which each fp16 test
+    that could overflow (|acc| <= 4K, row_scale up to 2) asserts on its data.
   * Attention: queries and keys built from digit codes route every query row to one target key with a logit gap of
-    >= 64 in log2 units; the softmax is one-hot far below bf16 resolution and the output IS the target's value row.
-    Poison keys (a higher logit than the target) sit just past the causal boundary and in the next batch's rows.
+    >= 64 in log2 units; the softmax is one-hot far below 16-bit resolution and the output IS the target's value row.
+    In bf16 the other keys' P (<= 2^-64) enters the P V MMA as a tiny normal number; in fp16 it underflows to exactly
+    0.  Poison keys (a higher logit than the target) sit just past the causal boundary and in the next batch's rows; in
+    fp16, whose largest finite value is 65504, the poison logit 2^21 is split as 2^15 * 2^6 over query and key.
 
 Where the exactness premise had to be narrowed, the test says so: the RoPE table is quantised to multiples of 2^-8, the
 routing tests use a softmax scale whose product with log2(e) is exactly 2^-3 (decode: scale 1/8).  The production
 table and the production scale 1 / sqrt(D) are covered by the bounded sections.
 
-Bounded sections: check_elementwise() against the bound each test derives.  Worst measured error / bound on one H100
-80GB HBM3: activation epilogues 0.98 (SwiGLU 0.95), production QKV epilogue 0.96, folded LayerNorm with row means of
-+-20..40 0.88, attention with logit std 1 / 4 / 16 0.77 / 0.85 / 0.79, patch embedding (CLIP form) 0.97.  The worst
-elements are those whose final bf16 rounding error is close to half an ulp just above a power of two, where the
-rounding term 2^-8 |ref| of the bound is tight; the fp32 terms add little."""
+Bounded sections: check_elementwise() against the bound each test derives; the rounding into the storage type is
+storage_bound: 2^-8 |x| for bf16, 2^-11 |x| + 2^-25 (half the subnormal spacing) for fp16.  attention_bound has, for
+fp16, a subnormal term 2^-25 sum_j |v_j|: the unnormalised P (<= 1) loses up to 2^-25 per key when it is rounded to fp16
+for the P V MMA.  Worst measured error / bound on one H100 80GB HBM3 (700 W power limit), bf16 / fp16: activation
+epilogues 0.98 / 0.91 (SwiGLU 0.95 / 0.80), production QKV epilogue 0.96 / 0.83, folded LayerNorm with row means of
++-20..40 0.88 / 0.64, attention with logit std 1 / 4 / 16 0.77 / 0.85 / 0.79 and 0.71 / 0.67 / 0.52, patch embedding
+(CLIP form) 0.97 / 0.95.  In bf16 the worst elements are those whose final rounding error is close to half an ulp just
+above a power of two, where the rounding term of the bound is tight and the fp32 terms add little; at fp16's 2^-11 the
+fp32 terms (accumulation, ex2, rsqrt) are a larger share of the bound, which the ratios stay clear of.
+
+fp16 only (section 4): the top of the range - 65504 stays, 65504 < x < 65520 becomes 65504, x >= 65520 becomes inf,
+as torch rounds, in the GEMM epilogue on single-CTA and pair tiles, with split-K and with a residual, and sumsq_out of
+an overflowed slot is inf; results in the subnormal range are the correctly rounded subnormals; subnormal operands
+enter the wgmma GEMM and attention (as V) unflushed."""
 import math
 
 import numpy as np
@@ -30,8 +47,42 @@ import torch
 pytestmark = pytest.mark.gpu
 
 LOG2E = 1.4426950408889634
-BF16_REL = 2.0 ** -8     # round-to-nearest into bf16 (8 significant bits): |rnd(x) - x| <= 2^-8 |x|
 F32_U = 2.0 ** -24       # fp32 unit roundoff
+FP16_MAX = 65504.0       # largest finite fp16; fp16 rounding sends |x| >= 65520 to inf
+
+# The two storage types the library builds for (libvl2.so, libvl2_f16.so).  Round-to-nearest into the type:
+# |rnd(x) - x| <= STORAGE_REL |x| + STORAGE_ABS, the absolute term being half the smallest subnormal spacing (fp16:
+# subnormals below 2^-14 are spaced 2^-24 apart; bf16 has the exponent range of fp32, so none arise in these tests).
+STORAGE_TYPES = (torch.bfloat16, torch.float16)
+STORAGE_BITS = {torch.bfloat16: 8, torch.float16: 11}                    # significant bits
+STORAGE_REL = {torch.bfloat16: 2.0 ** -8, torch.float16: 2.0 ** -11}
+STORAGE_ABS = {torch.bfloat16: 0.0, torch.float16: 2.0 ** -25}
+
+
+def _default_id(v, argname, idx):
+    """The id pytest gives parameter value v of argname at index idx when no ids are passed."""
+    if v is None or isinstance(v, (bool, int, float, str)):
+        return str(v)
+    return f"{argname}{idx}"
+
+
+def storage_params(argnames, values):
+    """parametrize over the storage type `dt` (first) and `argnames` / `values`.  The bf16 cases keep the
+    ids pytest gives `values` alone - the ids these tests had when they ran on bf16 only - and the fp16 cases are
+    'fp16-<that id>'."""
+    names = [n.strip() for n in argnames.split(",")]
+    cases = []
+    for dt in STORAGE_TYPES:
+        for i, v in enumerate(values):
+            vs = tuple(v) if len(names) > 1 else (v,)
+            vid = "-".join(_default_id(x, n, i) for x, n in zip(vs, names))
+            cases.append(pytest.param(dt, *vs, id=vid if dt == torch.bfloat16 else f"fp16-{vid}"))
+    return pytest.mark.parametrize(",".join(["dt"] + names), cases)
+
+
+def tag(dt) -> str:
+    """Prefix of the printed section names: none for bf16 (the names they always had), 'fp16 ' for fp16."""
+    return "" if dt == torch.bfloat16 else "fp16 "
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -70,37 +121,48 @@ def gemm_acc_bound(a: torch.Tensor, w: torch.Tensor) -> torch.Tensor:
     return math.ceil(K / 16) * 2.0 ** -21 * (a.double().abs() @ w.double().abs().t())
 
 
-def gemm_bf16_bound(ref: torch.Tensor, acc_err: torch.Tensor) -> torch.Tensor:
-    """A bf16 result: the fp32 errors carried into the final rounding plus that rounding (2^-8 of the value)."""
-    return BF16_REL * ref.double().abs() + (1 + BF16_REL) * acc_err + 1e-30
+def storage_bound(ref: torch.Tensor, acc_err: torch.Tensor, dt) -> torch.Tensor:
+    """A result of storage type dt: the fp32 errors carried into the final rounding plus that rounding (2^-8 of the
+    value for bf16; 2^-11 of the value plus 2^-25, half the fp16 subnormal spacing, for fp16)."""
+    u = STORAGE_REL[dt]
+    return u * ref.double().abs() + (1 + u) * acc_err + STORAGE_ABS[dt] + 1e-30
 
 
-def attention_bound(ref, p, v_abs, ds_max, s_abs_max, n_kv_tiles) -> torch.Tensor:
+def attention_bound(ref, p, v_abs, ds_max, s_abs_max, n_kv_tiles, dt, v_abs_sum=None) -> torch.Tensor:
     """Bound on one attention output element o = sum_j p_j v_j (p the exact softmax) of the wgmma kernel:
-      * P enters the P V MMA rounded to bf16 while l sums the fp32 values: <= 2^-8 sum p|v|;
+      * P enters the P V MMA rounded to the storage type while l sums the fp32 values: <= u sum p|v| (u = 2^-8 / 2^-11);
+        in fp16 every unnormalised p_j (<= 1, scaled by factors <= 1 afterwards, divided by l >= 1) may in addition lose
+        up to 2^-25 to a subnormal or zero: <= 2^-25 sum_j |v_j| over the visible keys (v_abs_sum);
       * logit errors ds (fp32 Q K^T, scaled) move every p by a relative <= 2 max ds: <= 2 ds_max sum p|v|;
       * ex2.approx and the fp32 rounding of its argument s * scale_log2 - m: relative <= 2^-21 (1 + |s scale_log2|);
       * fp32 accumulation of P V over the key tiles (8 k16 steps each): <= 8 n_kv 2^-21 sum p|v|;
-      * the bf16 output rounding."""
+      * the output rounding into the storage type."""
+    u = STORAGE_REL[dt]
     pv = p @ v_abs
-    rel = BF16_REL + 2 * ds_max + 2.0 ** -21 * (1 + s_abs_max) + 8 * n_kv_tiles * 2.0 ** -21
-    return BF16_REL * ref.abs() + (1 + BF16_REL) * rel * pv + 1e-30
+    rel = u + 2 * ds_max + 2.0 ** -21 * (1 + s_abs_max) + 8 * n_kv_tiles * 2.0 ** -21
+    bound = u * ref.abs() + (1 + u) * rel * pv + 1e-30
+    if STORAGE_ABS[dt]:
+        bound = bound + (1 + u) * STORAGE_ABS[dt] * v_abs_sum + STORAGE_ABS[dt]
+    return bound
 
 
-def attention_reference(q, k, v, causal, scale):
+def attention_reference(q, k, v, causal, scale, dt):
     """fp64 attention of q [H, S, D], k / v [H, S, D] (GQA already expanded) with everything attention_bound needs."""
     q, k, v = q.double(), k.double(), v.double()
     S, D = q.shape[1], q.shape[2]
     s = (q @ k.transpose(1, 2)) * scale
     ds = math.ceil(D / 16) * 2.0 ** -21 * (q.abs() @ k.abs().transpose(1, 2)) * scale
+    visible = torch.ones(S, S, dtype=torch.float64, device=q.device)
     if causal:
         mask = torch.ones(S, S, dtype=torch.bool, device=q.device).triu(1)
         s = s.masked_fill(mask, -math.inf)
         ds = ds.masked_fill(mask, 0.0)
+        visible = visible.masked_fill(mask, 0.0)
     p = torch.softmax(s, -1)
     ref = p @ v
     s_abs = torch.nan_to_num(s.abs(), posinf=0.0).amax(-1, keepdim=True) * LOG2E
-    bound = attention_bound(ref, p, v.abs(), ds.amax(-1, keepdim=True), s_abs, math.ceil(S / 128))
+    bound = attention_bound(ref, p, v.abs(), ds.amax(-1, keepdim=True), s_abs, math.ceil(S / 128), dt,
+                            v_abs_sum=visible @ v.abs())
     return ref, bound
 
 
@@ -112,21 +174,28 @@ def relerr(a, b):
 # ---------------------------------------------------------------------------------------------------------------------
 # inputs
 # ---------------------------------------------------------------------------------------------------------------------
-def ints(shape, lo, hi, seed, dev, dtype=torch.bfloat16):
+def ints(shape, lo, hi, seed, dev, dtype):
     g = torch.Generator(device=dev).manual_seed(seed)
     return torch.randint(lo, hi + 1, shape, generator=g, device=dev).to(dtype)
 
 
-def rnd(shape, dev, scale=1.0, seed=0, dtype=torch.bfloat16):
+def rnd(shape, dev, scale=1.0, seed=0, *, dtype):
     g = torch.Generator().manual_seed(seed)
     return (torch.randn(shape, generator=g) * scale).to(dtype).to(dev)
 
 
-def to_bf16_exact(ref64: torch.Tensor) -> torch.Tensor:
-    """Round an fp64 result that fp32 holds exactly to bf16 (nearest even), as the kernels' pack_bf16 does."""
+def to_storage_exact(ref64: torch.Tensor, dt) -> torch.Tensor:
+    """Round an fp64 result that fp32 holds exactly to the storage type dt (nearest even; fp16: subnormals kept, +-inf
+    from 65520 on), as the kernels' pack_bf16 / __float2bfloat16_rn do in the build for dt."""
     r32 = ref64.float()
     assert torch.equal(r32.double(), ref64), "exactness premise: the fp64 result must be fp32-exact"
-    return r32.to(torch.bfloat16)
+    return r32.to(dt)
+
+
+def storage_ulp(v: torch.Tensor, dt) -> torch.Tensor:
+    """The spacing of dt's values at |v| (fp16: at least the subnormal spacing 2^-24)."""
+    ulp = torch.ldexp(torch.ones_like(v), torch.frexp(v.float())[1].to(torch.int32) - STORAGE_BITS[dt])
+    return ulp if dt == torch.bfloat16 else ulp.clamp(min=2.0 ** -24)
 
 
 def assert_nan(t: torch.Tensor, what: str) -> None:
@@ -161,133 +230,157 @@ def _edge_cases(bn):
             (130, w + 8, 14336)]
 
 
-@pytest.mark.parametrize("bn", TILES)
-def test_gemm_exact_every_tile_and_edge(cuda, bn):
+def _assert_fp16_range(ref: torch.Tensor, what) -> None:
+    """Premise of the fp16 instances of the exact tests: no output reaches fp16's overflow threshold."""
+    assert float(ref.abs().max()) < FP16_MAX, f"{what}: the random data reaches the fp16 range"
+
+
+@storage_params("bn", TILES)
+def test_gemm_exact_every_tile_and_edge(cuda, dt, bn):
     """Operands in {-2..2} (|acc| <= 4K <= 57344): exact fp32 accumulation, so the output is the fp64 product rounded once.
-    Per tile shape and edge case: (a) bf16 output written into a column slice of a NaN-filled wider, taller buffer from a
-    row-strided A (lda > K), integer bias and power-of-two row_scale; (b) the output aliasing an integer residual in such
-    a buffer; (c) fp32 output.  Nothing outside the output slice may change."""
+    Per tile shape and edge case: (a) 16-bit output written into a column slice of a NaN-filled wider, taller buffer
+    from a row-strided A (lda > K), integer bias and power-of-two row_scale; (b) the output aliasing an integer residual
+    in such a buffer; (c) fp32 output.  Nothing outside the output slice may change.  In fp16, integers above 2048 round
+    (still one rounding of an fp32-exact value), and |acc| row_scale + bias could reach 2 * 57344 + 8 by construction;
+    the random sums have a standard deviation of 2 sqrt(K) <= 240 and stay far below 65504, which is asserted."""
     from videollama2_b200 import ops
     for ci, (M, N, K) in enumerate(_edge_cases(bn)):
         seed = 1000 * bn + 10 * ci
-        a_full = ints((M, K + 16), -2, 2, seed, cuda)
+        a_full = ints((M, K + 16), -2, 2, seed, cuda, dt)
         a = a_full[:, 8:8 + K]
-        w = ints((N, K), -2, 2, seed + 1, cuda)
+        w = ints((N, K), -2, 2, seed + 1, cuda, dt)
         bias = ints((N,), -8, 8, seed + 2, cuda, torch.float32)
         rs = (2.0 ** torch.randint(-2, 2, (M,), generator=torch.Generator().manual_seed(seed + 3))).float().to(cuda)
         acc = a.double() @ w.double().t()
-        tag = (bn, M, N, K)
+        tag_ = (bn, M, N, K)
         # (a)
-        buf = torch.full((M + 3, N + 32), float("nan"), device=cuda, dtype=torch.bfloat16)
+        buf = torch.full((M + 3, N + 32), float("nan"), device=cuda, dtype=dt)
         out = buf[:M, 16:16 + N]
         ops.gemm(a, w, bias=bias, row_scale=rs, out=out, bn=bn)
-        assert torch.equal(out, to_bf16_exact(acc * rs.double()[:, None] + bias.double())), ("bias/row_scale", tag)
-        assert_nan(buf[:, :16], f"left guard {tag}")
-        assert_nan(buf[:, 16 + N:], f"right guard {tag}")
-        assert_nan(buf[M:], f"rows past M {tag}")
+        ref = acc * rs.double()[:, None] + bias.double()
+        if dt == torch.float16:
+            _assert_fp16_range(ref, tag_)
+        assert torch.equal(out, to_storage_exact(ref, dt)), ("bias/row_scale", tag_)
+        assert_nan(buf[:, :16], f"left guard {tag_}")
+        assert_nan(buf[:, 16 + N:], f"right guard {tag_}")
+        assert_nan(buf[M:], f"rows past M {tag_}")
         # (b)
-        buf = torch.full((M + 3, N + 32), float("nan"), device=cuda, dtype=torch.bfloat16)
+        buf = torch.full((M + 3, N + 32), float("nan"), device=cuda, dtype=dt)
         view = buf[:M, 16:16 + N]
-        view.copy_(ints((M, N), -8, 8, seed + 4, cuda))
+        view.copy_(ints((M, N), -8, 8, seed + 4, cuda, dt))
         ref = acc + view.double()
         ops.gemm(a, w, residual=view, out=view, bn=bn)
-        assert torch.equal(view, to_bf16_exact(ref)), ("aliased residual", tag)
-        assert_nan(buf[:, :16], f"left guard (aliased) {tag}")
-        assert_nan(buf[:, 16 + N:], f"right guard (aliased) {tag}")
-        assert_nan(buf[M:], f"rows past M (aliased) {tag}")
+        assert torch.equal(view, to_storage_exact(ref, dt)), ("aliased residual", tag_)
+        assert_nan(buf[:, :16], f"left guard (aliased) {tag_}")
+        assert_nan(buf[:, 16 + N:], f"right guard (aliased) {tag_}")
+        assert_nan(buf[M:], f"rows past M (aliased) {tag_}")
         # (c)
         o32 = ops.gemm(a.contiguous(), w, out_dtype=torch.float32, bn=bn)
-        assert torch.equal(o32.double(), acc), ("fp32 output", tag)
+        assert torch.equal(o32.double(), acc), ("fp32 output", tag_)
 
 
-@pytest.mark.parametrize("M,N,K,bn", [
+@storage_params("M,N,K,bn", [
     (1776, 4096, 14336, 0),     # decoder down_proj
     (1776, 6144, 4096, 0),      # decoder QKV
     (1200, 4096, 2048, 256),    # single-CTA tiles: 160 tiles on 132 SMs
     (1154, 1024, 4096, 1128),   # ViT fc2 of a 2-frame shard on pair tiles
     (1776, 4096, 1024, 1256),   # short K: 16 k-blocks
 ])
-def test_gemm_splitk_bit_identical_to_unsplit(cuda, M, N, K, bn):
+def test_gemm_splitk_bit_identical_to_unsplit(cuda, dt, M, N, K, bn):
     """With exact arithmetic the split-K partials add the same products as the unsplit kernel: forced 2, 3 and 4 K-slices
-    are bit-identical to it, and to the fp64 product."""
+    are bit-identical to it, and to the fp64 product (fp16: the sums stay below 2048 + 8 * 2 sqrt(K) or so, far below
+    65504, asserted)."""
     from videollama2_b200 import ops
-    a = ints((M, K), -2, 2, 21, cuda)
-    w = ints((N, K), -2, 2, 22, cuda)
-    res = ints((M, N), -8, 8, 23, cuda)
-    ref = to_bf16_exact(a.double() @ w.double().t() + res.double())
+    a = ints((M, K), -2, 2, 21, cuda, dt)
+    w = ints((N, K), -2, 2, 22, cuda, dt)
+    res = ints((M, N), -8, 8, 23, cuda, dt)
+    ref64 = a.double() @ w.double().t() + res.double()
+    if dt == torch.float16:
+        _assert_fp16_range(ref64, (M, N, K))
+    ref = to_storage_exact(ref64, dt)
     unsplit = ops.gemm(a, w, residual=res, bn=bn, splitk=False)
     assert torch.equal(unsplit, ref)
     for s in (2, 3, 4):
         assert torch.equal(ops.gemm(a, w, residual=res, bn=bn, splitk=s), unsplit), s
 
 
-@pytest.mark.parametrize("bn", [0, 64, 96, 160, 256, 1128, 1192, 1256])
-def test_gemm_statistics_exact(cuda, bn):
-    """sumsq_out / rowsum_out on operands in {-1, 0, 1}: outputs are integers <= 200 (bf16-exact) and the per-32-column
-    sums of squares stay below 2^24, so both statistics equal the fp64 sums exactly."""
+@storage_params("bn", [0, 64, 96, 160, 256, 1128, 1192, 1256])
+def test_gemm_statistics_exact(cuda, dt, bn):
+    """sumsq_out / rowsum_out on operands in {-1, 0, 1}: outputs are integers <= 200 (exact in both storage types) and
+    the per-32-column sums of squares stay below 2^24, so both statistics equal the fp64 sums exactly."""
     from videollama2_b200 import ops
     M, N, K = 700, 1056, 192
-    a = ints((M, K), -1, 1, 31, cuda)
-    w = ints((N, K), -1, 1, 32, cuda)
-    res = ints((M, N), -8, 8, 33, cuda)
+    a = ints((M, K), -1, 1, 31, cuda, dt)
+    w = ints((N, K), -1, 1, 32, cuda, dt)
+    res = ints((M, N), -8, 8, 33, cuda, dt)
     sq = torch.full((M, N // 32), float("nan"), device=cuda)
     sm = torch.full((M, N // 32), float("nan"), device=cuda)
     out = ops.gemm(a, w, residual=res, sumsq_out=sq, rowsum_out=sm, bn=bn)
     ref = a.double() @ w.double().t() + res.double()
-    assert torch.equal(out, to_bf16_exact(ref))
+    assert torch.equal(out, to_storage_exact(ref, dt))
     assert torch.equal(sq.double(), (ref ** 2).view(M, N // 32, 32).sum(-1))
     assert torch.equal(sm.double(), ref.view(M, N // 32, 32).sum(-1))
 
 
-def _rope_table_quantised(n_pos, D, theta, dev):
-    """A RoPE table in the layout of ops.rope_table with cos / sin rounded to multiples of 2^-8.  The production table's
-    tiny sines (down to ~2^-20) would make x0 cos - x1 sin span more than fp32's 24 bits; on this grid the products of
-    integers with the table's 8-bit mantissas AND their sums are fp32-exact, whatever the compiler contracts."""
+def rope_table_bits(c: torch.Tensor, s: torch.Tensor) -> torch.Tensor:
+    """ops.rope_table's layout from 16-bit cos / sin tensors: cos in the low half, sin in the high half of an int32."""
+    return (c.view(torch.int16).to(torch.int32) & 0xFFFF) | (s.view(torch.int16).to(torch.int32) << 16)
+
+
+def _rope_table_quantised(n_pos, D, theta, dev, dt):
+    """A RoPE table in the layout of ops.rope_table with cos / sin rounded to multiples of 2^-8 (exact in bf16 and
+    fp16).  The production table's tiny sines (down to ~2^-20) would make x0 cos - x1 sin span more than fp32's 24
+    bits; on this grid the products of integers with the table's 8-bit mantissas AND their sums are fp32-exact,
+    whatever the compiler contracts."""
     inv = 1.0 / (theta ** (torch.arange(0, D, 2, dtype=torch.int64).double() / D))
     ang = torch.outer(torch.arange(n_pos, dtype=torch.float64), inv)
-    c = (torch.round(ang.cos() * 256) / 256).to(torch.bfloat16)
-    s = (torch.round(ang.sin() * 256) / 256).to(torch.bfloat16)
+    c = (torch.round(ang.cos() * 256) / 256).to(dt)
+    s = (torch.round(ang.sin() * 256) / 256).to(dt)
     assert torch.equal(c.double(), torch.round(ang.cos() * 256) / 256)
-    tab = (c.view(torch.int16).to(torch.int32) & 0xFFFF) | (s.view(torch.int16).to(torch.int32) << 16)
-    return tab.contiguous().to(dev), c.double().to(dev), s.double().to(dev)
+    return rope_table_bits(c, s).contiguous().to(dev), c.double().to(dev), s.double().to(dev)
 
 
-@pytest.mark.parametrize("bn", [0, 64, 128, 1256])
-def test_gemm_rope_epilogue_exact(cuda, bn):
-    """Integer projection + integer bias, rotated by a bf16 cos / sin table on adjacent column pairs (2i, 2i+1) of every
-    q / k head, v columns untouched: bit-exact against the fp64 rotation."""
+@storage_params("bn", [0, 64, 128, 1256])
+def test_gemm_rope_epilogue_exact(cuda, dt, bn):
+    """Integer projection + integer bias, rotated by a 16-bit cos / sin table on adjacent column pairs (2i, 2i+1) of
+    every q / k head, v columns untouched: bit-exact against the fp64 rotation (|rotated| <= 2 * 264 on the 2^-8 grid:
+    fp32-exact, one rounding into fp16)."""
     from videollama2_b200 import ops
     S, Hq, Hkv, D, pos0, K = 300, 4, 2, 128, 5, 64
     nqk, N = (Hq + Hkv) * D, (Hq + 2 * Hkv) * D
-    x = ints((S, K), -2, 2, 41, cuda)
-    w = ints((N, K), -2, 2, 42, cuda)
+    x = ints((S, K), -2, 2, 41, cuda, dt)
+    w = ints((N, K), -2, 2, 42, cuda, dt)
     b = ints((N,), -8, 8, 43, cuda, torch.float32)
-    tab, c, s = _rope_table_quantised(pos0 + S + 2, D, 1e6, cuda)
+    tab, c, s = _rope_table_quantised(pos0 + S + 2, D, 1e6, cuda, dt)
     out = ops.gemm(x, w, bias=b, rope=(tab, pos0, D, nqk), bn=bn)
     y = x.double() @ w.double().t() + b.double()
     qk = y[:, :nqk].view(S, Hq + Hkv, D // 2, 2)
     co, sn = c[pos0:pos0 + S][:, None, :], s[pos0:pos0 + S][:, None, :]
     rot = torch.stack([qk[..., 0] * co - qk[..., 1] * sn, qk[..., 1] * co + qk[..., 0] * sn], -1).reshape(S, nqk)
-    assert torch.equal(out, to_bf16_exact(torch.cat([rot, y[:, nqk:]], 1)))
+    assert torch.equal(out, to_storage_exact(torch.cat([rot, y[:, nqk:]], 1), dt))
 
 
 @pytest.mark.parametrize("pad", [1, 0])
-@pytest.mark.parametrize("T,H,W,C,N,bn", [(16, 24, 24, 4096, 512, 0), (4, 6, 6, 64, 64, 0), (8, 27, 27, 128, 256, 0),
-                                          (3, 5, 7, 64, 96, 0), (16, 24, 24, 256, 512, 1256), (16, 24, 24, 256, 512, 128),
-                                          (2, 30, 30, 64, 64, 0)])
-def test_conv3d_implicit_gemm_exact(cuda, T, H, W, C, N, bn, pad):
-    """The Conv3d(k = s = 2) front end on integer x / weights / bias (|acc| <= 4 * 8C <= 131072): bit-exact against fp64
+@storage_params("T,H,W,C,N,bn", [(16, 24, 24, 4096, 512, 0), (4, 6, 6, 64, 64, 0), (8, 27, 27, 128, 256, 0),
+                                 (3, 5, 7, 64, 96, 0), (16, 24, 24, 256, 512, 1256), (16, 24, 24, 256, 512, 128),
+                                 (2, 30, 30, 64, 64, 0)])
+def test_conv3d_implicit_gemm_exact(cuda, dt, T, H, W, C, N, bn, pad):
+    """The Conv3d(k = s = 2) front end on integer x / weights / bias (|acc| <= 4 * 8C <= 131072 by construction; the
+    random sums have a standard deviation of 2 sqrt(8C) <= 362, asserted below 65504 for fp16): bit-exact against fp64
     conv3d, including the zero-padded border taps and the padded output lines."""
     from videollama2_b200 import ops
     if (W % 2 == 1 or H % 2 == 1) and pad == 1:
         pytest.skip("odd H / W with padding is not a configuration of the path")
-    x = ints((T, H, W, C), -2, 2, 51, cuda)
-    wt = ints((N, C, 2, 2, 2), -2, 2, 52, cuda)
+    x = ints((T, H, W, C), -2, 2, 51, cuda, dt)
+    wt = ints((N, C, 2, 2, 2), -2, 2, 52, cuda, dt)
     b = ints((N,), -8, 8, 53, cuda, torch.float32)
     wk = wt.permute(0, 2, 3, 4, 1).reshape(N, 8 * C).contiguous()
     out = ops.conv3d_k2s2(x, wk, bias=b, pad=pad, bn=bn)
     ref = torch.nn.functional.conv3d(x.double().permute(3, 0, 1, 2)[None], wt.double(), b.double(), stride=2, padding=pad)
-    assert torch.equal(out, to_bf16_exact(ref[0].permute(1, 2, 3, 0).reshape(-1, N)))
+    ref = ref[0].permute(1, 2, 3, 0).reshape(-1, N)
+    if dt == torch.float16:
+        _assert_fp16_range(ref, (T, H, W, C, N))
+    assert torch.equal(out, to_storage_exact(ref, dt))
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -295,7 +388,13 @@ def test_conv3d_implicit_gemm_exact(cuda, T, H, W, C, N, bn, pad):
 # ---------------------------------------------------------------------------------------------------------------------
 L_CODE = 512.0          # query amplitude on its target's code: the target beats any other key by >= 512 logit units
 R_RAMP = 512.0          # logit step per key position of the ramp heads
-L_POISON = 2.0 ** 21    # poison channel: beats every legitimate logit (<= 512 * 1776)
+L_POISON = 2.0 ** 21    # poison logit: beats every legitimate logit (<= 512 * 1776)
+
+
+def poison_split(dt):
+    """(query, key) values of a poison channel with product L_POISON: bf16 holds 2^21 itself; fp16's largest finite value
+    is 65504, so there the query carries 2^15 and the key 2^6."""
+    return (L_POISON, 1.0) if dt == torch.bfloat16 else (2.0 ** 15, 2.0 ** 6)
 
 
 def _digits(u: torch.Tensor, nd: int) -> torch.Tensor:
@@ -307,8 +406,8 @@ def _code_onehot(u: torch.Tensor, nd: int) -> torch.Tensor:
     return torch.nn.functional.one_hot(_digits(u, nd), 4).flatten(-2).double()
 
 
-def _routing_problem(B, S, Hq, Hkv, D, causal):
-    """q / k / v [B, S, H, D] (fp64, bf16-exact) and the target key of every (batch, row, query head).
+def _routing_problem(B, S, Hq, Hkv, D, causal, dt):
+    """q / k / v [B, S, H, D] (fp64, exact in the storage type dt) and the target key of every (batch, row, query head).
 
     Layout of the D columns: [nd base-4 digit one-hots | ramp (2) | poison channels (B - 1) | zero].
       * Targets: up to 12 key positions spread over the first, middle and last key tiles, each with its own code.  A code
@@ -317,9 +416,10 @@ def _routing_problem(B, S, Hq, Hkv, D, causal):
       * Ramp heads (odd heads, causal only): logit = R_RAMP * key position, so the target is the diagonal key and every
         key past the boundary, i + 1 first, is a poison with a higher logit; the row maximum arrives in the last tile.
       * Batch poison: the first rows of batch b + 1 - those the TMA box of batch b's tail tile would reach in memory -
-        carry channel b, which every query of batch b weights with L_POISON."""
+        carry channel b, which every query of batch b weights so that the logit is L_POISON (poison_split)."""
     nd = (D - 2 - (B - 1)) // 4
     rb, pb = 4 * nd, 4 * nd + 2
+    pq, pk = poison_split(dt)
     n_t = min(4 ** nd, S, 12)
     tpos = torch.unique(torch.linspace(0, S - 1, n_t).round().long())
     n_t = tpos.numel()
@@ -335,7 +435,7 @@ def _routing_problem(B, S, Hq, Hkv, D, causal):
     q[..., rb] = 64 * R_RAMP * ramp
     q[..., rb + 1] = R_RAMP * ramp
     for b in range(B - 1):
-        q[b, ..., pb + b] = L_POISON
+        q[b, ..., pb + b] = pq
     target = torch.where(ramp, i.expand(B, S, Hq), tpos[u])
     k[:, tpos, :, :rb] = _code_onehot(torch.arange(n_t), nd)[None, :, None, :]
     j = torch.arange(S, dtype=torch.float64)
@@ -343,31 +443,22 @@ def _routing_problem(B, S, Hq, Hkv, D, causal):
     k[..., rb + 1] = (j % 64)[None, :, None]
     n_pad = min(S, -S % 128)
     for b in range(1, B):
-        k[b, :n_pad, :, pb + b - 1] = 1.0
-    v = torch.randn(B, S, Hkv, D, generator=torch.Generator().manual_seed(B * S + D)).to(torch.bfloat16).double()
+        k[b, :n_pad, :, pb + b - 1] = pk
+    v = torch.randn(B, S, Hkv, D, generator=torch.Generator().manual_seed(B * S + D)).to(dt).double()
     for t in (q, k):
-        assert torch.equal(t.to(torch.bfloat16).double(), t)
+        assert torch.equal(t.to(dt).double(), t)
     return q, k, v, target
 
 
-@pytest.mark.parametrize("B,S,Hq,Hkv,D,causal", [
-    (1, 1, 2, 2, 64, False), (1, 1, 2, 1, 128, True), (3, 2, 2, 2, 64, True), (3, 2, 4, 2, 8, False),
-    (1, 127, 4, 2, 128, True), (3, 127, 2, 2, 72, False), (1, 128, 2, 2, 64, False), (3, 128, 14, 2, 128, True),
-    (3, 129, 4, 4, 40, False), (1, 129, 28, 4, 128, True), (1, 255, 2, 1, 96, True), (3, 255, 4, 2, 64, False),
-    (3, 256, 7, 1, 64, True), (1, 256, 16, 16, 72, False), (3, 257, 28, 4, 128, True), (1, 257, 2, 2, 8, False),
-    (3, 45, 2, 2, 8, True), (3, 300, 6, 3, 40, True), (1, 1776, 28, 4, 128, True), (3, 1776, 8, 8, 64, False),
-    (1, 1776, 4, 2, 96, False), (3, 729, 16, 16, 72, False),
-])
-def test_attention_routing_exact(cuda, B, S, Hq, Hkv, D, causal):
-    """out[b, i, h] == v[b, target(b, i, h), h // group] bit for bit, with poison keys past the causal boundary and in
-    the next batch's rows, targets in the first / middle / last key tile (the online-softmax rescale runs whenever a
-    later tile raises the maximum), and the output written with ldo > Hq * D between NaN guard columns."""
+def _run_routing(cuda, dt, B, S, Hq, Hkv, D, causal, v=None):
+    """Run a routing problem (optionally with other value rows v [B, S, Hkv, D]) and check out == the target's row."""
     from videollama2_b200 import ops
-    q, k, v, target = _routing_problem(B, S, Hq, Hkv, D, causal)
+    q, k, v0, target = _routing_problem(B, S, Hq, Hkv, D, causal, dt)
+    v = v0 if v is None else v
     scale, _ = exact_softmax_scale()
     qkv = torch.cat([q.reshape(B * S, Hq * D), k.reshape(B * S, Hkv * D), v.reshape(B * S, Hkv * D)], 1)
-    qkv = qkv.to(torch.bfloat16).to(cuda)
-    buf = torch.full((B * S, Hq * D + 16), float("nan"), device=cuda, dtype=torch.bfloat16)
+    qkv = qkv.to(dt).to(cuda)
+    buf = torch.full((B * S, Hq * D + 16), float("nan"), device=cuda, dtype=dt)
     out = buf[:, 8:8 + Hq * D]
     ops.attention(qkv[:, :Hq * D], qkv[:, Hq * D:(Hq + Hkv) * D], qkv[:, (Hq + Hkv) * D:], B=B, S=S, Hq=Hq, Hkv=Hkv, D=D,
                   causal=causal, scale=scale, out=out)
@@ -380,9 +471,26 @@ def test_attention_routing_exact(cuda, B, S, Hq, Hkv, D, causal):
     assert_nan(buf[:, 8 + Hq * D:], "right guard")
 
 
+@storage_params("B,S,Hq,Hkv,D,causal", [
+    (1, 1, 2, 2, 64, False), (1, 1, 2, 1, 128, True), (3, 2, 2, 2, 64, True), (3, 2, 4, 2, 8, False),
+    (1, 127, 4, 2, 128, True), (3, 127, 2, 2, 72, False), (1, 128, 2, 2, 64, False), (3, 128, 14, 2, 128, True),
+    (3, 129, 4, 4, 40, False), (1, 129, 28, 4, 128, True), (1, 255, 2, 1, 96, True), (3, 255, 4, 2, 64, False),
+    (3, 256, 7, 1, 64, True), (1, 256, 16, 16, 72, False), (3, 257, 28, 4, 128, True), (1, 257, 2, 2, 8, False),
+    (3, 45, 2, 2, 8, True), (3, 300, 6, 3, 40, True), (1, 1776, 28, 4, 128, True), (3, 1776, 8, 8, 64, False),
+    (1, 1776, 4, 2, 96, False), (3, 729, 16, 16, 72, False),
+])
+def test_attention_routing_exact(cuda, dt, B, S, Hq, Hkv, D, causal):
+    """out[b, i, h] == v[b, target(b, i, h), h // group] bit for bit, with poison keys past the causal boundary and in
+    the next batch's rows, targets in the first / middle / last key tile (the online-softmax rescale runs whenever a
+    later tile raises the maximum), and the output written with ldo > Hq * D between NaN guard columns.  In fp16 the
+    other keys' P (<= 2^-64) underflows to exactly 0 when it is rounded for the P V MMA, where bf16 keeps it; l sums
+    the fp32 values (1 + <= 2^-64 * S == 1), so the output is the target's row in both types."""
+    _run_routing(cuda, dt, B, S, Hq, Hkv, D, causal)
+
+
 @pytest.mark.parametrize("D", [64, 128])
-@pytest.mark.parametrize("causal", [False, True])
-def test_attention_equal_top_logits_exact(cuda, D, causal):
+@storage_params("causal", [False, True])
+def test_attention_equal_top_logits_exact(cuda, dt, D, causal):
     """Two keys with equal top logits in different key tiles (positions 5 and 260): out = (v_a + v_b) / 2, bit for bit
     (values are integers of equal parity, so the mean is exact); causal rows 5..259 see only v_a (rows before 5 see no
     coded key and are not checked)."""
@@ -398,7 +506,7 @@ def test_attention_equal_top_logits_exact(cuda, D, causal):
     k[pb, :4] = 1.0
     v = torch.randint(-100, 101, (S, Hkv * D), generator=torch.Generator().manual_seed(7)).double()
     v[pb] -= (v[pa] + v[pb]) % 2
-    qkv = torch.cat([q, k, v], 1).to(torch.bfloat16).to(cuda)
+    qkv = torch.cat([q, k, v], 1).to(dt).to(cuda)
     out = ops.attention(qkv[:, :Hq * D], qkv[:, Hq * D:(Hq + Hkv) * D], qkv[:, (Hq + Hkv) * D:], B=1, S=S, Hq=Hq,
                         Hkv=Hkv, D=D, causal=causal, scale=scale)
     want = ((v[pa] + v[pb]) / 2).repeat(Hq)[None, :].expand(S, Hq * D).clone()
@@ -411,14 +519,16 @@ def _decode_nsplit(Hkv):
     return max(1, min(64, (2 * 148) // Hkv))      # decode.cu decode_nsplit: only used to place targets in every split
 
 
-@pytest.mark.parametrize("n_pos,Hq,Hkv,D", [(1, 4, 2, 128), (127, 8, 8, 64), (128, 28, 4, 128), (129, 32, 8, 128),
-                                            (5000, 14, 2, 128), (40000, 8, 1, 128), (40000, 16, 4, 64)])
-def test_attention_decode_routing_exact(cuda, n_pos, Hq, Hkv, D):
+@storage_params("n_pos,Hq,Hkv,D", [(1, 4, 2, 128), (127, 8, 8, 64), (128, 28, 4, 128), (129, 32, 8, 128),
+                                   (5000, 14, 2, 128), (40000, 8, 1, 128), (40000, 16, 4, 64)])
+def test_attention_decode_routing_exact(cuda, dt, n_pos, Hq, Hkv, D):
     """Split-KV decode attention routes each query head to its target key bit for bit: targets at position 0, at the last
     position and inside every split, a poison row at n_pos (one past the last visible position) and beyond; the graph
-    variant reading the position from device memory is bit-identical."""
+    variant reading the position from device memory is bit-identical.  (fp16: the other keys' weights underflow to 0,
+    as in test_attention_routing_exact.)"""
     from videollama2_b200 import ops
     nd = (D - 1) // 4
+    pq, pk = poison_split(dt)
     n_tiles = (n_pos + 127) // 128
     tpos = {0, n_pos - 1}
     for s in range(min(_decode_nsplit(Hkv), n_tiles)):
@@ -427,12 +537,12 @@ def test_attention_decode_routing_exact(cuda, n_pos, Hq, Hkv, D):
     n_t = tpos.numel()
     assert n_t <= 4 ** nd
     width = (Hq + 2 * Hkv) * D
-    cache = torch.zeros(n_pos + 3, width, dtype=torch.bfloat16, device=cuda)
+    cache = torch.zeros(n_pos + 3, width, dtype=dt, device=cuda)
     kc = cache[:, Hq * D:(Hq + Hkv) * D].view(n_pos + 3, Hkv, D)
-    kc[tpos.to(cuda), :, :4 * nd] = _code_onehot(torch.arange(n_t), nd)[:, None, :].to(cuda, torch.bfloat16)
-    kc[n_pos:, :, D - 1] = 1.0                                                  # poison: past the last position
+    kc[tpos.to(cuda), :, :4 * nd] = _code_onehot(torch.arange(n_t), nd)[:, None, :].to(cuda, dt)
+    kc[n_pos:, :, D - 1] = pk                                                   # poison: past the last position
     g = torch.Generator().manual_seed(n_pos + Hq)
-    cache[:, (Hq + Hkv) * D:] = torch.randn(n_pos + 3, Hkv * D, generator=g).to(torch.bfloat16).to(cuda)
+    cache[:, (Hq + Hkv) * D:] = torch.randn(n_pos + 3, Hkv * D, generator=g).to(dt).to(cuda)
     k, v = cache[:, Hq * D:(Hq + Hkv) * D], cache[:, (Hq + Hkv) * D:]
     vv = v.view(n_pos + 3, Hkv, D)
     pos_dev = torch.tensor([n_pos - 1], device=cuda, dtype=torch.int32)
@@ -441,8 +551,8 @@ def test_attention_decode_routing_exact(cuda, n_pos, Hq, Hkv, D):
         u = (call * Hq + torch.arange(Hq)) % n_t
         q = torch.zeros(Hq, D, dtype=torch.float64)
         q[:, :4 * nd] = L_CODE * _code_onehot(u, nd)
-        q[:, D - 1] = L_POISON
-        qd = q.reshape(-1).to(torch.bfloat16).to(cuda)
+        q[:, D - 1] = pq
+        qd = q.reshape(-1).to(dt).to(cuda)
         out = ops.attention_decode(qd, k, v, n_pos=n_pos, Hq=Hq, Hkv=Hkv, D=D, scale=0.125)
         want = vv[tpos[u].to(cuda), (torch.arange(Hq) // group).to(cuda)].reshape(1, Hq * D)
         bad = (out != want).view(Hq, D).any(-1).cpu()
@@ -454,6 +564,15 @@ def test_attention_decode_routing_exact(cuda, n_pos, Hq, Hkv, D):
 
 def test_attention_decode_equal_top_logits_exact(cuda):
     """Two keys with equal top logits in different decode splits: the combine step returns (v_a + v_b) / 2 exactly."""
+    _decode_equal_top_logits(cuda, torch.bfloat16)
+
+
+def test_attention_decode_equal_top_logits_exact_fp16(cuda):
+    """test_attention_decode_equal_top_logits_exact on the fp16 build."""
+    _decode_equal_top_logits(cuda, torch.float16)
+
+
+def _decode_equal_top_logits(cuda, dt):
     from videollama2_b200 import ops
     n_pos, Hq, Hkv, D = 5000, 8, 2, 128
     pa, pb = 70, 128 * 5 + 3                          # tiles 0 and 5: different splits
@@ -464,9 +583,9 @@ def test_attention_decode_equal_top_logits_exact(cuda):
     vals = torch.randint(-100, 101, (n_pos, Hkv * D), generator=torch.Generator().manual_seed(3)).double()
     vals[pb] -= (vals[pa] + vals[pb]) % 2
     cache[:, (Hq + Hkv) * D:] = vals
-    cd = cache.to(torch.bfloat16).to(cuda)
+    cd = cache.to(dt).to(cuda)
     # logit 64 * 128 * scale = 1024 nats over the zero keys: their exp underflows to exactly 0
-    q = torch.full((Hq * D,), 64.0, device=cuda, dtype=torch.bfloat16)
+    q = torch.full((Hq * D,), 64.0, device=cuda, dtype=dt)
     out = ops.attention_decode(q, cd[:, Hq * D:(Hq + Hkv) * D], cd[:, (Hq + Hkv) * D:], n_pos=n_pos, Hq=Hq, Hkv=Hkv, D=D,
                                scale=0.125)
     want = ((vals[pa] + vals[pb]) / 2).view(Hkv, D).repeat_interleave(Hq // Hkv, 0).reshape(1, -1)
@@ -492,15 +611,15 @@ def _act_rel(x):
 
 
 @pytest.mark.parametrize("bn", [64, 160, 256, 1128, 1224])
-@pytest.mark.parametrize("act", [1, 2, 3, 5, 4])   # 4 = SwiGLU
-def test_gemm_activation_epilogues_bounded(cuda, bn, act):
+@storage_params("act", [1, 2, 3, 5, 4])   # 4 = SwiGLU
+def test_gemm_activation_epilogues_bounded(cuda, dt, bn, act):
     """Every activation and SwiGLU on single-CTA and pair tiles, each element within its bound: the accumulation
     (gemm_acc_bound, times the row scale and the activation's slope), the fp32 bias add, the activation's own
-    approximation, the bf16 output rounding."""
+    approximation, the output rounding."""
     from videollama2_b200 import ops
     M, N, K = 600, 528, 320
-    a = rnd((M, K), cuda, seed=61)
-    w = rnd((N, K), cuda, 0.08, seed=62)
+    a = rnd((M, K), cuda, seed=61, dtype=dt)
+    w = rnd((N, K), cuda, 0.08, seed=62, dtype=dt)
     bias = torch.randn(N, generator=torch.Generator().manual_seed(63)).to(cuda)
     acc = a.double() @ w.double().t()
     e_acc = gemm_acc_bound(a, w)
@@ -519,20 +638,21 @@ def test_gemm_activation_epilogues_bounded(cuda, bn, act):
         ex = e_acc * rs.double()[:, None] + 2 * F32_U * (x.abs() + bias.double().abs())
         ref = ACT64[act](x)
         err = ACT_SLOPE * ex + _act_rel(x) * ref.abs()
-    check_elementwise(out, ref, gemm_bf16_bound(ref, err), f"act {act} bn {bn}", tile=(256 if bn > 1000 else 128, bn % 1000))
+    check_elementwise(out, ref, storage_bound(ref, err, dt), f"{tag(dt)}act {act} bn {bn}",
+                      tile=(256 if bn > 1000 else 128, bn % 1000))
 
 
-@pytest.mark.parametrize("bn", [0, 64, 1256])
-def test_gemm_qkv_production_epilogue_bounded(cuda, bn):
+@storage_params("bn", [0, 64, 1256])
+def test_gemm_qkv_production_epilogue_bounded(cuda, dt, bn):
     """The decoder's QKV projection as it runs (decoder._layer): folded RMSNorm (rms_in from row_sumsq) + bias + RoPE with
-    the production bf16 table, in one epilogue; element-wise against fp64."""
+    the production table of the storage type, in one epilogue; element-wise against fp64."""
     from videollama2_b200 import ops
     S, Hq, Hkv, D, K, pos0 = 300, 4, 2, 128, 512, 17
     nqk, N = (Hq + Hkv) * D, (Hq + 2 * Hkv) * D
-    x = rnd((S, K), cuda, 2.0, seed=71)
-    w = rnd((N, K), cuda, K ** -0.5, seed=72)
+    x = rnd((S, K), cuda, 2.0, seed=71, dtype=dt)
+    w = rnd((N, K), cuda, K ** -0.5, seed=72, dtype=dt)
     b = rnd((N,), cuda, 0.5, seed=73, dtype=torch.float32)
-    tab = ops.rope_table(pos0 + S, D, 1e6, cuda)
+    tab = ops.rope_table(pos0 + S, D, 1e6, cuda, dt)
     ss = ops.row_sumsq(x)
     out = ops.gemm(x, w, bias=b, rms_in=ss, rms_eps=1e-5, rope=(tab, pos0, D, nqk), bn=bn)
     xd = x.double()
@@ -542,8 +662,8 @@ def test_gemm_qkv_production_epilogue_bounded(cuda, bn):
     # rs: fp32 sum of squares (<= K 2^-24 relative, any order), rsqrtf (2 ulp): relative <= K 2^-25 + 2^-21
     ey = gemm_acc_bound(x, w) * rs + (K * 2.0 ** -25 + 2.0 ** -21) * (acc * rs).abs() + 2 * F32_U * (y.abs() + b.double().abs())
     tv = tab.cpu()
-    c = (tv & 0xFFFF).to(torch.int16).view(torch.bfloat16).double()[pos0:pos0 + S].to(cuda)
-    s = (tv >> 16).to(torch.int16).view(torch.bfloat16).double()[pos0:pos0 + S].to(cuda)
+    c = (tv & 0xFFFF).to(torch.int16).view(dt).double()[pos0:pos0 + S].to(cuda)
+    s = (tv >> 16).to(torch.int16).view(dt).double()[pos0:pos0 + S].to(cuda)
     yq, eq = y[:, :nqk].view(S, Hq + Hkv, D // 2, 2), ey[:, :nqk].view(S, Hq + Hkv, D // 2, 2)
     co, sn = c[:, None, :], s[:, None, :]
     r0 = yq[..., 0] * co - yq[..., 1] * sn
@@ -552,11 +672,11 @@ def test_gemm_qkv_production_epilogue_bounded(cuda, bn):
         + 2 * F32_U * (yq[..., 0].abs() + yq[..., 1].abs())
     ref = torch.cat([torch.stack([r0, r1], -1).reshape(S, nqk), y[:, nqk:]], 1)
     err = torch.cat([torch.stack([e_rot, e_rot], -1).reshape(S, nqk), ey[:, nqk:]], 1)
-    check_elementwise(out, ref, gemm_bf16_bound(ref, err), f"qkv bn {bn}")
+    check_elementwise(out, ref, storage_bound(ref, err, dt), f"{tag(dt)}qkv bn {bn}")
 
 
-@pytest.mark.parametrize("bn", [0, 64, 1128])
-def test_gemm_folded_layernorm_large_mean_bounded(cuda, bn):
+@storage_params("bn", [0, 64, 1128])
+def test_gemm_folded_layernorm_large_mean_bounded(cuda, dt, bn):
     """Folded LayerNorm rstd * (x W'^T - mu * colsum) + b' on rows with mean and std ~ 30 (the outlier channels of CLIP
     residual streams): the cancellation in acc - mu * colsum and in E[x^2] - mu^2 must stay within the bound built from
     the accumulation (which scales with |x|, i.e. with the mean), the fp32 row statistics and the fp32 column sums."""
@@ -564,8 +684,8 @@ def test_gemm_folded_layernorm_large_mean_bounded(cuda, bn):
     M, K, N = 577, 1024, 1024
     g = torch.Generator().manual_seed(81)
     mu_row = (torch.rand(M, 1, generator=g) * 20 + 20) * torch.where(torch.rand(M, 1, generator=g) < 0.5, -1.0, 1.0)
-    x = (mu_row + 30 * torch.randn(M, K, generator=g)).to(torch.bfloat16).to(cuda)
-    wf = rnd((N, K), cuda, K ** -0.5, seed=82)
+    x = (mu_row + 30 * torch.randn(M, K, generator=g)).to(dt).to(cuda)
+    wf = rnd((N, K), cuda, K ** -0.5, seed=82, dtype=dt)
     colsum = wf.double().sum(1)
     bias = rnd((N,), cuda, 0.2, seed=83, dtype=torch.float32)
     stats = ops.row_stats(x)
@@ -583,23 +703,23 @@ def test_gemm_folded_layernorm_large_mean_bounded(cuda, bn):
     d_rstd = d_var / (2 * (var + 1e-5)) + 2.0 ** -21                                  # relative, rsqrtf 2 ulp
     e_cen = gemm_acc_bound(x, wf) + (mu.abs() * F32_U + d_mu) * colsum.abs()[None, :] + F32_U * (acc.abs() + (mu * colsum).abs())
     err = rstd * e_cen + d_rstd * (rstd * cen).abs() + 2 * F32_U * (ref.abs() + bias.double().abs())
-    check_elementwise(out, ref, gemm_bf16_bound(ref, err), f"folded LN bn {bn}")
+    check_elementwise(out, ref, storage_bound(ref, err, dt), f"{tag(dt)}folded LN bn {bn}")
 
 
 @pytest.mark.parametrize("sigma", [1.0, 4.0, 16.0])
-@pytest.mark.parametrize("B,S,Hq,Hkv,D,causal", [(2, 577, 4, 4, 64, False), (1, 1776, 8, 2, 128, True),
-                                                 (3, 300, 6, 2, 72, True)])
-def test_attention_peaky_logits_bounded(cuda, sigma, B, S, Hq, Hkv, D, causal):
+@storage_params("B,S,Hq,Hkv,D,causal", [(2, 577, 4, 4, 64, False), (1, 1776, 8, 2, 128, True), (3, 300, 6, 2, 72, True)])
+def test_attention_peaky_logits_bounded(cuda, dt, sigma, B, S, Hq, Hkv, D, causal):
     """Logit standard deviation sigma (q, k ~ N(0, sqrt(sigma)), production scale 1 / sqrt(D)); causal rows get a ramp
     of 3 sigma over the key positions, so the row maximum tends to arrive in a late key tile and the running maximum is
-    raised tile after tile.  Every output element within attention_bound."""
+    raised tile after tile.  Every output element within attention_bound.  sigma = 16 puts most of P below 2^-14, i.e.
+    into fp16's subnormal range, where the subnormal term of attention_bound is the one that counts."""
     from videollama2_b200 import ops
     amp = math.sqrt(sigma)
-    qkv = rnd((B * S, (Hq + 2 * Hkv) * D), cuda, amp, seed=int(sigma) * 7 + D)
+    qkv = rnd((B * S, (Hq + 2 * Hkv) * D), cuda, amp, seed=int(sigma) * 7 + D, dtype=dt)
     if causal:
         qkv[:, :Hq * D].view(B * S, Hq, D)[:, :, 0] = math.sqrt(D)
         ramp = (3 * sigma * torch.arange(S, device=cuda) / S).repeat(B)
-        qkv[:, Hq * D:(Hq + Hkv) * D].view(B * S, Hkv, D)[:, :, 0] = ramp[:, None].to(torch.bfloat16)
+        qkv[:, Hq * D:(Hq + Hkv) * D].view(B * S, Hkv, D)[:, :, 0] = ramp[:, None].to(dt)
     scale = D ** -0.5
     q, k, v = qkv[:, :Hq * D], qkv[:, Hq * D:(Hq + Hkv) * D], qkv[:, (Hq + Hkv) * D:]
     out = ops.attention(q, k, v, B=B, S=S, Hq=Hq, Hkv=Hkv, D=D, causal=causal, scale=scale)
@@ -610,17 +730,18 @@ def test_attention_peaky_logits_bounded(cuda, sigma, B, S, Hq, Hkv, D, causal):
         qf = q[rows].view(S, Hq, D).transpose(0, 1)
         kf = k[rows].view(S, Hkv, D).transpose(0, 1).repeat_interleave(G, 0)
         vf = v[rows].view(S, Hkv, D).transpose(0, 1).repeat_interleave(G, 0)
-        ref, bound = attention_reference(qf, kf, vf, causal, scale)
+        ref, bound = attention_reference(qf, kf, vf, causal, scale, dt)
         got = out[rows].view(S, Hq, D).transpose(0, 1)
         for h in range(Hq):
-            worst = max(worst, check_elementwise(got[h], ref[h], bound[h], f"sigma {sigma} batch {b} head {h}",
+            worst = max(worst, check_elementwise(got[h], ref[h], bound[h], f"{tag(dt)}sigma {sigma} batch {b} head {h}",
                                                  tile=(128, D)))
-    print(f"worst error/bound attention sigma {sigma} {(B, S, Hq, Hkv, D, causal)}: {worst:.3f}")
+    print(f"worst error/bound {tag(dt)}attention sigma {sigma} {(B, S, Hq, Hkv, D, causal)}: {worst:.3f}")
 
 
 def _ln_rows_bound(x, d_x, gamma, beta):
     """fp64 LayerNorm of rows x [R, C] (gamma, beta [C]) and a bound on the kernel's fp32 result given per-element input
-    errors d_x: fp32 row sums (<= C 2^-24 of the sums of |terms|), E[x^2] - mu^2, rsqrtf, the normalise-scale-shift."""
+    errors d_x: fp32 row sums (<= C 2^-24 of the sums of |terms|), E[x^2] - mu^2, rsqrtf, the normalise-scale-shift.
+    The rounding into the storage type is storage_bound's."""
     C = x.shape[1]
     mu = x.mean(-1, keepdim=True)
     var = x.var(-1, unbiased=False, keepdim=True)
@@ -634,30 +755,30 @@ def _ln_rows_bound(x, d_x, gamma, beta):
     return y, err
 
 
-@pytest.mark.parametrize("F,H,P,C", [(2, 56, 14, 128), (3, 112, 14, 256), (16, 336, 14, 1024), (2, 336, 14, 1024)])
-def test_patch_embed_clip_rowwise_bounded(cuda, F, H, P, C):
-    """CLIP form (conv rounded to bf16 -> + position -> pre-LayerNorm; class row LN(cls + pos[0]) in every frame) checked
-    row by row at C = 128 / 256 / 1024, i.e. clusters of 1, 2, 4 and 8 CTAs sharing a row's LayerNorm statistics over
-    distributed shared memory.  Where the fp32 conv sum may round to the other side of a bf16 midpoint than the exact
-    sum, one bf16 ulp of input error is allowed for that element."""
+@storage_params("F,H,P,C", [(2, 56, 14, 128), (3, 112, 14, 256), (16, 336, 14, 1024), (2, 336, 14, 1024)])
+def test_patch_embed_clip_rowwise_bounded(cuda, dt, F, H, P, C):
+    """CLIP form (conv rounded to the storage type -> + position -> pre-LayerNorm, as in HF; class row LN(cls + pos[0])
+    in every frame) checked row by row at C = 128 / 256 / 1024, i.e. clusters of 1, 2, 4 and 8 CTAs sharing a row's
+    LayerNorm statistics over distributed shared memory.  Where the fp32 conv sum may round to the other side of a
+    rounding midpoint of the storage type than the exact sum, one ulp of input error is allowed for that element."""
     from videollama2_b200 import ops
-    px = rnd((F, 3, H, H), cuda, seed=91)
-    wconv = rnd((C, 3, P, P), cuda, 0.05, seed=92)
+    px = rnd((F, 3, H, H), cuda, seed=91, dtype=dt)
+    wconv = rnd((C, 3, P, P), cuda, 0.05, seed=92, dtype=dt)
     K = 3 * P * P
     Kpad = (K + 63) // 64 * 64
-    wpad = torch.zeros((C, Kpad), device=cuda, dtype=torch.bfloat16)
+    wpad = torch.zeros((C, Kpad), device=cuda, dtype=dt)
     wpad[:, :K] = wconv.reshape(C, K)
     npch = (H // P) ** 2
-    cls = rnd((C,), cuda, seed=93)
-    pos = rnd((npch + 1, C), cuda, seed=94)
-    g = rnd((C,), cuda, 0.1, seed=95) + 1
-    b = rnd((C,), cuda, 0.1, seed=96)
+    cls = rnd((C,), cuda, seed=93, dtype=dt)
+    pos = rnd((npch + 1, C), cuda, seed=94, dtype=dt)
+    g = rnd((C,), cuda, 0.1, seed=95, dtype=dt) + 1
+    b = rnd((C,), cuda, 0.1, seed=96, dtype=dt)
     tok = ops.patch_embed(px, wpad, pos, P, cls=cls, gamma=g, beta=b, eps=1e-5)
     A = torch.nn.functional.unfold(px.double(), kernel_size=P, stride=P).transpose(1, 2).reshape(-1, K)
     conv = A @ wconv.reshape(C, K).double().t()
     e_conv = math.ceil(Kpad / 16) * 2.0 ** -21 * (A.abs() @ wconv.reshape(C, K).double().abs().t())
-    conv_b = conv.float().to(torch.bfloat16).double()
-    ulp = torch.ldexp(torch.ones_like(conv), torch.frexp(conv.float())[1].to(torch.int32) - 8)
+    conv_b = conv.float().to(dt).double()
+    ulp = storage_ulp(conv, dt)
     mid_dist = ((conv - conv_b).abs() - ulp / 2).abs()                           # distance to the nearest rounding midpoint
     d_conv = torch.where(mid_dist <= e_conv, ulp, torch.zeros_like(ulp))
     x = torch.cat([(cls.double() + pos[0].double()).expand(F, 1, C),
@@ -665,23 +786,133 @@ def test_patch_embed_clip_rowwise_bounded(cuda, F, H, P, C):
     d_x = torch.cat([torch.zeros(F, 1, C, device=cuda, dtype=torch.float64), d_conv.view(F, npch, C)], 1).reshape(-1, C) \
         + F32_U * x.abs()
     ref, err = _ln_rows_bound(x, d_x, g.double(), b.double())
-    check_elementwise(tok, ref, gemm_bf16_bound(ref, err), f"patch embed C {C} F {F}", tile=(npch + 1, C))
+    check_elementwise(tok, ref, storage_bound(ref, err, dt), f"{tag(dt)}patch embed C {C} F {F}", tile=(npch + 1, C))
 
 
-@pytest.mark.parametrize("F,H,P,C", [(2, 384, 14, 1152), (3, 70, 14, 288)])
-def test_patch_embed_siglip_exact(cuda, F, H, P, C):
+@storage_params("F,H,P,C", [(2, 384, 14, 1152), (3, 70, 14, 288)])
+def test_patch_embed_siglip_exact(cuda, dt, F, H, P, C):
     """SigLIP form on integer pixels, weights, bias and positions (|acc| <= 4 * 588): conv + bias + position is exact in
     fp32, so the output is the fp64 result rounded once, bit for bit."""
     from videollama2_b200 import ops
-    px = ints((F, 3, H, H), -2, 2, 101, cuda)
-    wconv = ints((C, 3, P, P), -2, 2, 102, cuda)
+    px = ints((F, 3, H, H), -2, 2, 101, cuda, dt)
+    wconv = ints((C, 3, P, P), -2, 2, 102, cuda, dt)
     K = 3 * P * P
     Kpad = (K + 63) // 64 * 64
-    wpad = torch.zeros((C, Kpad), device=cuda, dtype=torch.bfloat16)
+    wpad = torch.zeros((C, Kpad), device=cuda, dtype=dt)
     wpad[:, :K] = wconv.reshape(C, K)
     npch = (H // P) ** 2
-    pos = ints((npch, C), -8, 8, 103, cuda)
+    pos = ints((npch, C), -8, 8, 103, cuda, dt)
     bias = ints((C,), -8, 8, 104, cuda, torch.float32)
     tok = ops.patch_embed(px, wpad, pos, P, bias=bias)
     patch = torch.nn.functional.conv2d(px.double(), wconv.double(), bias.double(), stride=P).flatten(2).transpose(1, 2)
-    assert torch.equal(tok, to_bf16_exact((patch + pos.double()).reshape(-1, C)))
+    assert torch.equal(tok, to_storage_exact((patch + pos.double()).reshape(-1, C), dt))
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# 4. fp16 only: the top of the range and the subnormals
+# ---------------------------------------------------------------------------------------------------------------------
+H16 = torch.float16
+# fp32 biases at the top of fp16's range: bias + (an integer accumulator of a few tens) crosses 65504 (kept), 65504..65520
+# (rounds down to 65504, e.g. 65519.75), 65520 (the midpoint to the next binade: +inf) and beyond, at both signs
+OVERFLOW_BIAS = [65504.0, 65504.75, 65496.25, 65520.0, 65536.0, 1.0e5, 65472.0, 0.0]
+
+
+def assert_overflow_classes(ref64: torch.Tensor) -> None:
+    """The fp64 results of an overflow test contain every case at both signs: exactly 65504, strictly between 65504 and
+    65520 (rounds to 65504), and >= 65520 (rounds to inf)."""
+    for sgn in (1.0, -1.0):
+        r = ref64 * sgn
+        assert bool((r == FP16_MAX).any()), "no result of exactly 65504"
+        assert bool(((r > FP16_MAX) & (r < 65520.0)).any()), "no result in (65504, 65520)"
+        assert bool((r >= 65520.0).any()), "no result >= 65520"
+
+
+@pytest.mark.parametrize("bn,splitk,residual", [(128, False, False), (1256, False, False), (128, 2, False),
+                                                (128, False, True), (1256, False, True), (0, 4, True)])
+def test_fp16_gemm_overflow_rounds_like_torch(cuda, bn, splitk, residual):
+    """Results at the top of fp16's range leave the epilogue (pack_bf16 = __floats2half2_rn in the fp16 build) as torch
+    rounds the fp64 result: 65504 stays, 65519.75 becomes 65504, 65520 and more become +-inf; no saturation, no NaN.
+    Integer accumulators in [-48, 48] plus fp32 biases of OVERFLOW_BIAS (or, with a residual, bias 0.75 and residuals
+    of +-65504 / +-65472) make every fp64 result fp32-exact.  Single-CTA and pair tiles, forced split-K, residual.  The
+    per-32-column sumsq_out of a slot holding an infinity is +inf, because the statistics are taken from the rounded
+    value the consumer reads, and finite otherwise."""
+    from videollama2_b200 import ops
+    M, N, K = 300, 256, 256
+    a = ints((M, K), -1, 1, 201, cuda, H16)
+    w = ints((N, K), -1, 1, 202, cuda, H16)
+    acc = a.double() @ w.double().t()
+    col = torch.arange(N)
+    big = (col // 32) % 2 == 0              # even 32-column slots reach the top of the range, odd ones stay moderate
+    sgn = torch.where(col % 2 == 0, 1.0, -1.0).double()
+    if residual:
+        bias = torch.where((col // 4) % 2 == 0, 0.0, 0.75).double()
+        res = sgn * torch.where(big, torch.tensor([FP16_MAX, 65472.0]).double()[(col // 2) % 2], 1000.0)
+        res = res[None, :].expand(M, N).to(H16).to(cuda).contiguous()
+        ref = acc + bias.to(cuda) + res.double()
+    else:
+        bias = sgn * torch.where(big, torch.tensor(OVERFLOW_BIAS).double()[(col // 2) % len(OVERFLOW_BIAS)], 1000.25)
+        res = None
+        ref = acc + bias.to(cuda)
+    assert_overflow_classes(ref)
+    sq = torch.full((M, N // 32), float("nan"), device=cuda)
+    out = ops.gemm(a, w, bias=bias.float().to(cuda), residual=res, sumsq_out=sq, bn=bn, splitk=splitk or False)
+    want = to_storage_exact(ref, H16)
+    assert not bool(torch.isnan(out).any()) and not bool(torch.isnan(sq).any())
+    assert torch.equal(out, want)
+    slot_inf = torch.isinf(want).view(M, N // 32, 32).any(-1)
+    assert torch.equal(torch.isinf(sq), slot_inf) and bool(slot_inf.any()) and bool((~slot_inf).any())
+    assert bool((sq[slot_inf] > 0).all())
+
+
+@pytest.mark.parametrize("bn", [128, 1256])
+def test_fp16_gemm_subnormal_results_rounded(cuda, bn):
+    """row_scale 2^-20 .. 2^-28 on integer accumulators: acc * row_scale (fp32-exact) lands in fp16's subnormal range
+    [2^-24, 2^-14) and below; the output must be torch's correctly rounded fp16 subnormal (round to nearest even on the
+    2^-24 grid), not zero and not a truncation."""
+    from videollama2_b200 import ops
+    M, N, K = 300, 256, 128
+    a = ints((M, K), -2, 2, 211, cuda, H16)
+    w = ints((N, K), -2, 2, 212, cuda, H16)
+    rs = (2.0 ** -torch.arange(20, 29)[torch.arange(M) % 9]).float().to(cuda)
+    acc = a.double() @ w.double().t()
+    ref = acc * rs.double()[:, None]
+    out = ops.gemm(a, w, row_scale=rs, bn=bn)
+    want = to_storage_exact(ref, H16)
+    sub = (want != 0) & (want.abs() < 2.0 ** -14)
+    assert int(sub.sum()) > 1000 and bool((want.double() != ref).any())      # subnormal results, many of them rounded
+    assert torch.equal(out, want)
+
+
+def subnormals(shape, kmax, seed, dev):
+    """fp16 subnormals k 2^-24, k in [-kmax, kmax] (zero included; kmax < 1024), as an fp16 tensor."""
+    g = torch.Generator().manual_seed(seed)
+    return (torch.randint(-kmax, kmax + 1, shape, generator=g).double() * 2.0 ** -24).to(H16).to(dev)
+
+
+@pytest.mark.parametrize("bn", [128, 1256])
+def test_fp16_gemm_subnormal_operands_exact(cuda, bn):
+    """Both wgmma operands fp16 subnormals (k 2^-24, |k| <= 63): their products k k' 2^-48 and sums (|sum k k'| <
+    192 * 2^12 < 2^24) are fp32-exact normals; row_scale 2^40 scales them to multiples of 2^-8 (fp32 output: exact),
+    2^24 to multiples of 2^-24 (fp16 output: one rounding, the smallest ones subnormal).  A flushed operand would give
+    zeros."""
+    from videollama2_b200 import ops
+    M, N, K = 300, 256, 192
+    a = subnormals((M, K), 63, 221, cuda)
+    w = subnormals((N, K), 63, 222, cuda)
+    assert bool((a != 0).any()) and float(a.abs().max()) < 2.0 ** -14
+    acc = a.double() @ w.double().t()
+    rs = torch.full((M,), 2.0 ** 40, device=cuda)
+    o32 = ops.gemm(a, w, row_scale=rs, out_dtype=torch.float32, bn=bn)
+    assert torch.equal(o32.double(), acc * 2.0 ** 40)
+    o16 = ops.gemm(a, w, row_scale=torch.full((M,), 2.0 ** 24, device=cuda), bn=bn)
+    assert torch.equal(o16, to_storage_exact(acc * 2.0 ** 24, H16))
+
+
+def test_fp16_attention_subnormal_values_exact(cuda):
+    """Value rows of fp16 subnormals through the routing problem: P is one-hot (1 on the target, 0 after the fp16
+    rounding elsewhere), so the output is the target's subnormal value row bit for bit; a flushed V operand or a flushed
+    output would give zeros."""
+    B, S, Hq, Hkv, D = 3, 300, 6, 3, 40
+    g = torch.Generator().manual_seed(231)
+    v = torch.randint(-1023, 1024, (B, S, Hkv, D), generator=g).double() * 2.0 ** -24
+    _run_routing(cuda, H16, B, S, Hq, Hkv, D, True, v=v)

@@ -1,12 +1,14 @@
 """Frame preprocessing (SURVEY.md §8f row 3): the numpy oracle against Pillow itself and the committed goldens, the
 product's host tables against the oracle's, frame_sample against the reference's outputs; on the GPU the CUDA resampler
 must reproduce Pillow's uint8 image bit for bit and the bf16 pixel_values must be the bf16 rounding of the reference's
-float32 values."""
+float32 values, and the fp16 pixel_values (the reference calls .half() on them) its fp16 rounding."""
 import os
 
 import numpy as np
 import pytest
 import torch
+
+from test_kernels_exact_gpu import storage_params
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "preprocess.pt")
 GOLD_HD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "preprocess_hd.pt")   # the 640 x 360 case
@@ -92,23 +94,33 @@ class _Proc:
 
 @pytest.mark.gpu
 def test_gpu_preprocess_matches_goldens(gold, cuda):
+    _preprocess_matches_goldens(gold, cuda, torch.bfloat16)
+
+
+@pytest.mark.gpu
+def test_gpu_preprocess_matches_goldens_fp16(gold, cuda):
+    """fp16 pixel_values (the reference calls .half() on them): the fp16 rounding of the goldens' float32 values."""
+    _preprocess_matches_goldens(gold, cuda, torch.float16)
+
+
+def _preprocess_matches_goldens(gold, cuda, dt):
     from videollama2_b200 import preprocess as pp
     for name, c in gold["cases"].items():
         proc = _Proc(c["kind"], c["size"])
         out, u8 = pp.preprocess_frames(c["frames"].to(cuda), c["size"], proc.image_mean, proc.image_std, kind=c["kind"],
-                                       aspect_ratio=c["aspect_ratio"], return_u8=True)
+                                       aspect_ratio=c["aspect_ratio"], return_u8=True, dtype=dt)
         assert torch.equal(u8.cpu(), c["u8"]), name                              # Pillow's uint8 image, bit for bit
-        assert out.shape == (c["T"], 3, c["size"], c["size"]) and out.dtype == torch.bfloat16
+        assert out.shape == (c["T"], 3, c["size"], c["size"]) and out.dtype == dt
         if c["pixel_values"] is not None:
-            assert torch.equal(out.cpu(), c["pixel_values"].to(torch.bfloat16)), name
+            assert torch.equal(out.cpu(), c["pixel_values"].to(dt)), name
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("H,W,size,kind,ar", [(1080, 1920, 336, "clip", "pad"), (720, 1280, 384, "siglip", "pad"),
-                                             (480, 854, 336, "clip", "resize"), (1920, 1080, 336, "clip", "pad"),
-                                             (336, 336, 336, "clip", "pad"), (100, 60, 336, "clip", "pad")])
-def test_gpu_preprocess_full_size_vs_oracle(cuda, H, W, size, kind, ar):
-    """Real frame sizes against the numpy oracle (which is pinned to Pillow above)."""
+@storage_params("H,W,size,kind,ar", [(1080, 1920, 336, "clip", "pad"), (720, 1280, 384, "siglip", "pad"),
+                                     (480, 854, 336, "clip", "resize"), (1920, 1080, 336, "clip", "pad"),
+                                     (336, 336, 336, "clip", "pad"), (100, 60, 336, "clip", "pad")])
+def test_gpu_preprocess_full_size_vs_oracle(cuda, dt, H, W, size, kind, ar):
+    """Real frame sizes against the numpy oracle (which is pinned to Pillow above), bf16 and fp16 pixel_values."""
     from oracle import preprocess_ref as P
     from videollama2_b200 import preprocess as pp
     rng = np.random.default_rng(H * 7 + W)
@@ -118,9 +130,9 @@ def test_gpu_preprocess_full_size_vs_oracle(cuda, H, W, size, kind, ar):
     proc = _Proc(kind, size)
     ref_u8, ref_px = P.preprocess_frames(list(frames), size, kind, ar)
     out, u8 = pp.preprocess_frames(torch.from_numpy(frames).to(cuda), size, proc.image_mean, proc.image_std, kind=kind,
-                                   aspect_ratio=ar, return_u8=True)
+                                   aspect_ratio=ar, return_u8=True, dtype=dt)
     assert np.array_equal(u8.cpu().numpy(), ref_u8)
-    assert torch.equal(out.cpu(), torch.from_numpy(ref_px).to(torch.bfloat16))
+    assert out.dtype == dt and torch.equal(out.cpu(), torch.from_numpy(ref_px).to(dt))
 
 
 @pytest.mark.gpu

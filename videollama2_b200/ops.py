@@ -288,13 +288,15 @@ def gemv(x: torch.Tensor, w: torch.Tensor, *, bias: Optional[torch.Tensor] = Non
 
 def attention_decode(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, *, n_pos: int, Hq: int, Hkv: int,
                      D: int, scale: float, out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """q [Hq*D]; k_cache / v_cache: row-strided views [>=n_pos, Hkv*D] of the per-layer cache."""
-    _need_cuda(q, k_cache, v_cache)
-    _bf16(q, k_cache, v_cache)
+    """q [Hq*D]; k_cache / v_cache: row-strided views [>=n_pos, Hkv*D] of the per-layer cache; out: Hq*D contiguous
+    elements of the storage type."""
+    _need_cuda(q, k_cache, v_cache, out)
+    _bf16(q, k_cache, v_cache, out)
     assert q.is_contiguous() and q.numel() == Hq * D and k_cache.stride(1) == 1 and v_cache.stride(1) == 1
     assert k_cache.stride(0) == v_cache.stride(0) and k_cache.shape[0] >= n_pos
     if out is None:
         out = torch.empty((1, Hq * D), device=q.device, dtype=q.dtype)
+    assert out.is_contiguous() and out.numel() == Hq * D, "attention_decode: out holds Hq * D contiguous elements"
     ws = decode_workspace(q.device, Hq, Hkv, D)
     check(_L(k_cache).vl2_attention_decode(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), out.data_ptr(),
                                            k_cache.stride(0), n_pos, Hq, Hkv, D, float(scale), ws.data_ptr(), _stream()),
@@ -304,13 +306,13 @@ def attention_decode(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tens
 
 def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, *, B: int, S: int, Hq: int, Hkv: int, D: int,
               causal: bool, scale: float, out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """q/k/v: 2-D row-strided views [B*S, H*D] (e.g. column slices of a fused QKV buffer)."""
+    """q/k/v/out: 2-D row-strided views [B*S, H*D] (e.g. column slices of a fused QKV buffer)."""
     _need_cuda(q, k, v, out)
-    _bf16(q, k, v)
-    for t, h in ((q, Hq), (k, Hkv), (v, Hkv)):
-        assert t.dim() == 2 and t.shape == (B * S, h * D) and t.stride(1) == 1
+    _bf16(q, k, v, out)
     if out is None:
         out = torch.empty((B * S, Hq * D), device=q.device, dtype=q.dtype)
+    for t, h in ((q, Hq), (k, Hkv), (v, Hkv), (out, Hq)):
+        assert t.dim() == 2 and t.shape == (B * S, h * D) and t.stride(1) == 1
     args = AttnArgs(q=q.data_ptr(), k=k.data_ptr(), v=v.data_ptr(), out=out.data_ptr(), ldq=q.stride(0),
                     ldk=k.stride(0), ldv=v.stride(0), ldo=out.stride(0), B=B, S=S, Hq=Hq, Hkv=Hkv, D=D,
                     causal=1 if causal else 0, scale=float(scale), reserved=0)
@@ -325,6 +327,7 @@ def decode_rope_append(qkv_row: torch.Tensor, cache: torch.Tensor, pos_dev: torc
     _bf16(qkv_row, cache)
     assert qkv_row.is_contiguous() and qkv_row.numel() == (Hq + 2 * Hkv) * D and cache.stride(1) == 1
     assert pos_dev.dtype == torch.int32 and pos_dev.numel() == 1
+    assert inv_freq.dtype == torch.float32 and inv_freq.numel() == D // 2
     check(_L(qkv_row).vl2_decode_rope_append(qkv_row.data_ptr(), cache.data_ptr(), cache.stride(0), pos_dev.data_ptr(),
                                              Hq, Hkv, D, inv_freq.data_ptr(), 1 if interleaved else 0, _stream()),
           "vl2_decode_rope_append")
