@@ -144,9 +144,13 @@ typedef struct vl2_gemm_args {
   int32_t rope_cols, rope_D, rope_pos0, reserved5;
 } vl2_gemm_args;
 int vl2_gemm_bf16(const vl2_gemm_args* args, void* stream);
-/* Debug aid: with args->reserved2 == 777 the first consumer thread of CTA 0 records clock64() at its tile boundaries:
- * out[0] = tiles traced (<= 7), and for tile t: out[8t+4] = starts the tile's k-loop, out[8t+5] = accumulator complete,
- * out[8t+6] = its part of the tile stored.  host_out128: 128 values.  Synchronises the device. */
+/* Debug aid: with args->reserved2 == 777 (or 779) the first consumer thread of CTA 0 records clock64() at its tile
+ * boundaries: out[0] = tiles traced (<= 7), and for tile t: out[8t+4] = starts the tile's k-loop, out[8t+5] = accumulator
+ * complete, out[8t+6] = its part of the tile stored.  Inside the tile's first 32-column slot: out[8t+1] = its accumulators
+ * selected and out[8t+2] = its residuals loaded (generic epilogue; -1 when a specialised variant ran), out[8t+3] = the
+ * slot stored.
+ * args->reserved2 == 778 (779 with the trace) forces the generic epilogue instead of the launch's specialised variant
+ * (tests: the results are the same bits).  host_out128: 128 values.  Synchronises the device. */
 int vl2_debug_gemm_trace(long long* host_out128);
 /* How many CTAs (pair = 0) or two-CTA clusters (pair = 1) of the GEMM kernel with tile width bn the current device runs at
  * once (occupancy API at the kernel's shared-memory size).  The persistent grid of vl2_gemm_bf16 is min(tiles, SMs) CTAs or

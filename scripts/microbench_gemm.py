@@ -9,8 +9,13 @@ tiles) gives per tile the k-loop cycles (start -> accumulator complete), the sam
 (accumulator complete -> stored).  The tensor pipe's bound for one k-block of a 128 x BN tile is 128 * BN * 64 MACs at
 2048 MACs per clock per SM, i.e. 4 * BN cycles.
 
-Usage: python scripts/microbench_gemm.py [--reps R] [--iters N] [--json FILE]
-       VL2_LIBVL2=/path/to/libvl2.so selects another build of the library (to compare two builds).
+Inside the first 32-column slot of a tile the trace also records (generic epilogue only) the accumulators selected and
+the residuals loaded, and (every epilogue) the slot stored: `slot0_cyc` = [select, residual round trip, whole slot].
+
+Usage: python scripts/microbench_gemm.py [--reps R] [--iters N] [--json FILE] [--generic]
+       --generic forces the library's generic epilogue instead of each launch's specialised variant.
+       VL2_LIBVL2=/path/to/libvl2.so selects another build of the library (to compare two builds; --generic and the
+       slot trace need a build that has them).
 """
 import argparse
 import ctypes as C
@@ -90,11 +95,12 @@ def main():
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--json", default=None)
+    ap.add_argument("--generic", action="store_true")
     args = ap.parse_args()
     dev = torch.device("cuda:0")
     lib = _lib.load()
     props = torch.cuda.get_device_properties(dev)
-    info = {"lib": _lib.LIB_PATH, "device": props.name, "sms": props.multi_processor_count}
+    info = {"lib": _lib.LIB_PATH, "device": props.name, "sms": props.multi_processor_count, "generic": args.generic}
     if hasattr(lib, "vl2_gemm_coresident"):   # absent from builds older than the query
         lib.vl2_gemm_coresident.argtypes = [C.c_int, C.c_int, C.c_void_p]
         res = C.c_int32()
@@ -109,6 +115,8 @@ def main():
     rows = []
     for k, rec in seen.items():
         a, w, kw = rec["a"], rec["w"], rec["kw"]
+        if args.generic:
+            kw = dict(kw, generic_epilogue=True)
         M, N, K = k[0], k[1], k[2]
         ops.check(lib.vl2_gemm_plan(M, N, K, 0, plan), "vl2_gemm_plan")
         bn, pair = plan[0], plan[1]
@@ -136,12 +144,15 @@ def main():
         tiles = [(t[8 * i + 4], t[8 * i + 5], t[8 * i + 6]) for i in range(int(t[0]))]
         kloop = [acc - st for st, acc, _ in tiles]
         epi = [done - acc for _, acc, done in tiles]
+        # first slot of each tile: [accumulators selected, residuals loaded, slot stored] after the accumulator is complete
+        slot0 = [[t[8 * i + j] - t[8 * i + 5] if t[8 * i + j] >= t[8 * i + 5] else None for j in (1, 2, 3)]
+                 for i in range(int(t[0]))]
         row = {"M": M, "N": N, "K": K, "epilogue": "+".join([f"act{k[3]}"] * (k[3] != 0) + [x for x in k[4:] if x]) or "-",
                "act": k[3], "calls_per_step": rec["calls"], "bn": bn, "pair": pair,
                "us": round(us, 1), "TFs": round(flop / us / 1e6, 1), "cublas_us": round(us_cub, 1),
                "cublas_TFs": round(flop / us_cub / 1e6, 1), "frac_of_cublas": round(us_cub / us, 3),
                "kb_per_tile": nkb, "mma_bound_cyc_per_kb": 4 * bn,
-               "kloop_cyc_per_kb": [round(c / nkb) for c in kloop], "epi_cyc": epi}
+               "kloop_cyc_per_kb": [round(c / nkb) for c in kloop], "epi_cyc": epi, "slot0_cyc": slot0}
         rows.append(row)
         print(json.dumps(row), flush=True)
 

@@ -79,9 +79,10 @@ def gemm(a: torch.Tensor, w: torch.Tensor, *, bias: Optional[torch.Tensor] = Non
          bcast_ptrs: Optional[list] = None, mc_ptr: int = 0, rms_in: Optional[torch.Tensor] = None,
          rms_eps: float = 0.0, sumsq_out: Optional[torch.Tensor] = None, trace: bool = False,
          splitk=True, ln_in=None, ln_colsum: Optional[torch.Tensor] = None,
-         rowsum_out: Optional[torch.Tensor] = None, rope=None) -> torch.Tensor:
+         rowsum_out: Optional[torch.Tensor] = None, rope=None, generic_epilogue: bool = False) -> torch.Tensor:
     """out[M,Nout] = epi(a[M,K] @ w[N,K]^T); a/w may be row-strided views (last dim contiguous).
-    `bn` forces the tile width (tests); 0 = library heuristic.
+    `bn` forces the tile width (tests); 0 = library heuristic.  `generic_epilogue` forces the library's generic
+    epilogue instead of the launch's specialised variant (tests compare the two; the results are the same bits).
     `bcast_ptrs`: device pointers of peer buffers (same layout as `out`) that receive every output vector too
     (epilogue-fused all-gather over NVLink); `mc_ptr`: NVSwitch multicast address used instead when non-zero.
     `rms_in` (fp32 [M, parts] partial row sums of squares of `a`) scales row m by rsqrt(sum(rms_in[m])/K + rms_eps):
@@ -164,8 +165,8 @@ def gemm(a: torch.Tensor, w: torch.Tensor, *, bias: Optional[torch.Tensor] = Non
             args.bcast_out[i] = ptr
         args.n_bcast = len(ptrs)
         args.mc_out = mc_ptr or None
-    if trace:
-        args.reserved2 = 777
+    if trace or generic_epilogue:
+        args.reserved2 = 779 if (trace and generic_epilogue) else (777 if trace else 778)
     forced = splitk is not True and splitk and int(splitk) > 1
     if forced or (splitk and _SPLITK_ENV):          # the workspace exists only when the split-K tail can actually run
         if forced:
@@ -192,10 +193,11 @@ def _splitk_workspace(device) -> torch.Tensor:
     return ws
 
 
-def gemm_trace() -> list:
-    """Tile-boundary cycle trace of the last gemm(..., trace=True) launch (vl2_debug_gemm_trace)."""
+def gemm_trace(dtype: torch.dtype = torch.bfloat16) -> list:
+    """Tile-boundary cycle trace of the last gemm(..., trace=True) launch (vl2_debug_gemm_trace) on operands of storage
+    type `dtype` (each storage-type build of the library keeps its own trace)."""
     buf = (C.c_longlong * 128)()
-    check(_lib.load().vl2_debug_gemm_trace(buf), "vl2_debug_gemm_trace")
+    check(_lib.load(dtype).vl2_debug_gemm_trace(buf), "vl2_debug_gemm_trace")
     return list(buf)
 
 
