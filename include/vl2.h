@@ -222,6 +222,30 @@ int vl2_attention_decode_dyn(const void* q, const void* k_cache, const void* v_c
                              const int32_t* pos_dev, int Hq, int Hkv, int D, float scale, void* workspace, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Token sampling for generate(do_sample=True): HF's TemperatureLogitsWarper -> TopKLogitsWarper -> TopPLogitsWarper ->
+ * softmax -> multinomial (transformers generation/logits_process.py, restated by videollama2_b200/sampling.py), one launch,
+ * graph-capturable.  logits fp32 [V], V <= 262144.  s = l / T (IEEE fp32 division); top-k (0 < top_k < V) keeps s >= the
+ * k-th largest s counting duplicates; top-p (top_p < 1) drops a token when the probability mass of the kept tokens
+ * strictly above it is >= top_p (ties at the boundary kept or dropped together; the maximum always stays); the token is
+ * the first kept index whose running sum of exp(s - max) exceeds u * (the kept sum), u = (x0 >> 8) * 2^-24 with x0 the
+ * first word of Philox4x32-10(counter = (n_lo, n_hi, 0, 0), key = (seed_lo, seed_hi)) and n = *counter_dev + counter_add.
+ * -inf / NaN scores and weights below 2^-41 of the maximum's are never drawn; a row with nothing drawable gives the first
+ * index of its maximum.  The parameters are read from device memory, so one captured graph serves every setting; no
+ * value in them changes which memory the kernel touches.  Deterministic: integer (fixed-point) sums only.
+ * ---------------------------------------------------------------------------------------------------------- */
+typedef struct vl2_sample_params {
+  float temperature;
+  float top_p;
+  int32_t top_k;
+  int32_t reserved;
+  uint64_t seed;
+} vl2_sample_params;
+/* logits 4-byte aligned; params, counter_dev and token_out 8-byte aligned (VL2_E_BADALIGN); V outside [1, 262144]:
+ * VL2_E_BADSHAPE. */
+int vl2_sample_token(const float* logits, int V, const vl2_sample_params* params, const int64_t* counter_dev,
+                     int64_t counter_add, int64_t* token_out, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Row-wise normalisations (HBM-bound, one pass).
  * vl2_layernorm: y = act( LN(x; gamma, beta, eps) [+ residual] )  over the last dim C (bf16 in/out, fp32 math).
  *   act in {NONE, SILU}; with residual the order is act(LN(x) + residual)   (timm Bottleneck: act3(conv3(..)+shortcut)).

@@ -77,7 +77,9 @@ def build_messages(instruct, modal: str, model_type: str):
 
 def mm_infer(image_or_video, instruct, model, tokenizer, modal="video", **kwargs):
     """Inference API of the reference (videollama2/__init__.py:39-114) on the H100 engine: prompt construction and
-    stopping criteria on the host (exact), vision + prefill + graph-replayed decode on the device.  Greedy only."""
+    stopping criteria on the host (exact), vision + prefill + graph-replayed decode on the device.  Greedy by default;
+    do_sample=True samples on the device (vl2_sample_token) with the reference's defaults: temperature 0.2, top_p 0.9 and
+    GenerationConfig's top_k 50; torch.manual_seed makes the draws reproducible."""
     import torch
     from .mm_utils import KeywordsStoppingCriteria, tokenizer_multimodal_token
     message, modal_token = build_messages(instruct, modal, model.config.model_type)

@@ -18,6 +18,7 @@ SYMBOLS = [
     "vl2_patch_im2col", "vl2_clip_embed_finish",
     "vl2_dwconv3x3_ln_silu", "vl2_se_scale", "vl2_conv3d_im2col",
     "vl2_rope_inplace", "vl2_embed_splice", "vl2_tp_allreduce_stats", "vl2_patch_embed",
+    "vl2_sample_token",
 ]
 
 ACT_NONE, ACT_QUICK_GELU, ACT_SILU, ACT_GELU_ERF, ACT_SWIGLU, ACT_GELU_TANH = 0, 1, 2, 3, 4, 5
@@ -68,6 +69,11 @@ class PatchEmbedArgs(C.Structure):
         ("F", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("P", C.c_int32), ("C", C.c_int32), ("Kpad", C.c_int32),
         ("eps", C.c_float), ("reserved", C.c_int32),
     ]
+
+
+class SampleParams(C.Structure):
+    _fields_ = [("temperature", C.c_float), ("top_p", C.c_float), ("top_k", C.c_int32), ("reserved", C.c_int32),
+                ("seed", C.c_uint64)]
 
 
 class Vl2Error(RuntimeError):
@@ -135,6 +141,7 @@ def load(dtype=None) -> C.CDLL:
         "vl2_embed_splice": [vp, vp, i32, vp, i64, vp, i32, vp],
         "vl2_tp_allreduce_stats": [C.POINTER(TpAllReduceArgs), vp],
         "vl2_patch_embed": [C.POINTER(PatchEmbedArgs), vp],
+        "vl2_sample_token": [vp, i32, vp, vp, i64, vp, vp],
     }
     for name, argtypes in sigs.items():
         fn = getattr(lib, name)

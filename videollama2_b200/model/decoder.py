@@ -1,4 +1,4 @@
-"""Mistral-7B / Qwen2 decoder prefill (+ greedy decode) on libvl2 kernels.
+"""Mistral-7B / Qwen2 decoder prefill (+ greedy or sampled decode) on libvl2 kernels.
 
 Arithmetic of HF MistralModel / Qwen2Model (HF:mistral/modeling_mistral.py:35-48,51-82,122-239,262-470;
 HF:qwen2/modeling_qwen2.py:187-246): RMSNorm -> fused QKV GEMM (+bias for Qwen2) -> RoPE -> causal GQA flash attention
@@ -32,8 +32,12 @@ class DecoderEngine:
         self.kv: List[torch.Tensor] = []   # per layer [S_max, (Hq+2Hkv)*D] fused qkv rows (K,V columns = cache)
         self.kv_len = 0
         self._graphed = None
-        self._decode_graph = None   # (graph, tok_dev, pos_dev, logits) of the captured single-token step
-        self._decode_log = None     # (device id buffer, device step counter) the graph appends its arg-max tokens to
+        self._decode_graph = None   # (graph, tok_dev, pos_dev, logits, stage) of the captured greedy single-token step
+        self._decode_graph_sampled = None   # the same step ending in vl2_sample_token instead of the arg-max
+        self._decode_bufs = None    # (tok_dev, pos_dev, stage, gen_buf, step_dev): device state both graphs share
+        self._decode_log = None     # (device id buffer, device step counter) the graphs append their tokens to
+        self._sample_params = None  # device vl2_sample_params the sampled graph reads (values copied in when armed)
+        self._armed = None          # the graph decode_graph_begin armed last
         self._decode_read = 0
         self.graph_decode = False
         self.decode_pdl = os.environ.get("VL2_DECODE_PDL", "0") == "1"   # PDL edges inside the decode graph
@@ -47,8 +51,12 @@ class DecoderEngine:
         from ..graphs import GraphedStage
         self._graphed = GraphedStage(lambda e: self._prefill_last(e)) if on else None
         self.graph_decode = on
-        self._decode_graph = None
+        self._drop_decode_graphs()
         return self
+
+    def _drop_decode_graphs(self) -> None:
+        """Forget both captured decode steps: they hold the addresses of the KV cache they were captured on."""
+        self._decode_graph = self._decode_graph_sampled = self._decode_bufs = self._armed = None
 
     def _prefill_last(self, embeds: torch.Tensor) -> torch.Tensor:
         return self.prefill(embeds, all_logits=False, keep_cache=False, _no_graph=True)[0]
@@ -159,7 +167,7 @@ class DecoderEngine:
         cap = (cap + 255) // 256 * 256
         width = (self.Hq + 2 * self.Hkv) * self.D
         self.kv = [torch.empty((cap, width), device=device, dtype=self.dtype) for _ in self.layers]
-        self._decode_graph = None
+        self._drop_decode_graphs()
 
     # ---- KV-cache decode (one token) -----------------------------------------------------------------------
     def decode_step(self, x: torch.Tensor) -> torch.Tensor:
@@ -186,9 +194,13 @@ class DecoderEngine:
         return ops.gemv(x, self.w["lm_head"], rms_eps=self.eps, out_dtype=torch.float32)
 
     # ---- the same step as ONE CUDA graph ---------------------------------------------------------------------
-    def _decode_body(self, tok_dev: torch.Tensor, pos_dev: torch.Tensor, stage: torch.Tensor, log=None) -> torch.Tensor:
+    def _decode_body(self, tok_dev: torch.Tensor, pos_dev: torch.Tensor, stage: torch.Tensor, log=None,
+                     sampler: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Single-token step whose position and token live in device memory: embeds *tok_dev, appends K/V at *pos_dev,
-        writes argmax(logits) back to tok_dev and increments pos_dev, so one captured graph serves every token."""
+        writes argmax(logits) back to tok_dev and increments pos_dev, so one captured graph serves every token.
+        `sampler` (a device vl2_sample_params block, needs `log`): the new token is drawn by vl2_sample_token with
+        counter *step_dev + 1 instead - the n-th new token of a generate() call uses counter n, token 0 came from the
+        prefill."""
         Hq, Hkv, D = self.Hq, self.Hkv, self.D
         x = torch.index_select(self.w["embed"], 0, tok_dev)
         o = torch.empty((1, Hq * D), device=x.device, dtype=self.dtype)
@@ -220,7 +232,10 @@ class DecoderEngine:
             h = ops.gemv(x, L["wgu"], act=ops.ACT_SWIGLU, rms_eps=self.eps)
             x = ops.gemv(h, L["wd"], residual=x)
         logits = ops.gemv(x, self.w["lm_head"], rms_eps=self.eps, out_dtype=torch.float32)
-        tok_dev.copy_(torch.argmax(logits, dim=1))
+        if sampler is None:
+            tok_dev.copy_(torch.argmax(logits, dim=1))
+        else:
+            ops.sample_token(logits, sampler, log[1], 1, tok_dev, self.dtype)
         pos_dev.add_(1)
         if log is not None:          # device-side log of the generated ids: the host reads it in chunks, not per token
             gen_buf, step_dev = log
@@ -228,34 +243,51 @@ class DecoderEngine:
             step_dev.add_(1)
         return logits
 
-    def decode_graph_begin(self, first_token: int) -> None:
-        """Arm the graph-replayed decode loop after prefill(keep_cache=True): token := first_token, pos := kv_len."""
+    def _capture_decode(self, sampler: Optional[torch.Tensor]):
+        """Capture the single-token step (greedy, or sampled with the parameter block `sampler`) on the shared buffers."""
+        dev = self.kv[0].device
+        if self._decode_bufs is None:
+            self._decode_bufs = (torch.zeros((1,), device=dev, dtype=torch.int64),
+                                 torch.zeros((1,), device=dev, dtype=torch.int32),
+                                 torch.empty((1, (self.Hq + 2 * self.Hkv) * self.D), device=dev, dtype=self.dtype),
+                                 torch.zeros((self.kv[0].shape[0] + 1,), device=dev, dtype=torch.int64),
+                                 torch.zeros((1,), device=dev, dtype=torch.int64))
+            self._decode_log = self._decode_bufs[3:]
+        tok_dev, pos_dev, stage, _, step_dev = self._decode_bufs
+        log = self._decode_log
+        scratch_pos = self.kv[0].shape[0] - 1     # warm-up writes land in the last cache row (rewritten when reached)
+        side = torch.cuda.Stream(device=dev)
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):
+            for _ in range(2):
+                pos_dev.fill_(scratch_pos)
+                step_dev.zero_()
+                with ops.pdl(self.decode_pdl):
+                    self._decode_body(tok_dev, pos_dev, stage, log, sampler)
+        torch.cuda.current_stream().wait_stream(side)
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph), ops.pdl(self.decode_pdl):
+            logits = self._decode_body(tok_dev, pos_dev, stage, log, sampler)
+        return (graph, tok_dev, pos_dev, logits, stage)
+
+    def decode_graph_begin(self, first_token: int, sampling: Optional[torch.Tensor] = None) -> None:
+        """Arm the graph-replayed decode loop after prefill(keep_cache=True): token := first_token, pos := kv_len.
+        `sampling`: an ops.sampling_params block - arm the sampled graph (captured once, then reused for every parameter
+        setting) instead of the greedy one."""
         if not self.kv:
             raise RuntimeError("decode_graph_begin needs prefill(keep_cache=True) first")
-        dev = self.kv[0].device
-        if self._decode_graph is None:
-            tok_dev = torch.zeros((1,), device=dev, dtype=torch.int64)
-            pos_dev = torch.zeros((1,), device=dev, dtype=torch.int32)
-            stage = torch.empty((1, (self.Hq + 2 * self.Hkv) * self.D), device=dev, dtype=self.dtype)
-            gen_buf = torch.zeros((self.kv[0].shape[0] + 1,), device=dev, dtype=torch.int64)
-            step_dev = torch.zeros((1,), device=dev, dtype=torch.int64)
-            log = (gen_buf, step_dev)
-            scratch_pos = self.kv[0].shape[0] - 1     # warm-up writes land in the last cache row (rewritten when reached)
-            side = torch.cuda.Stream(device=dev)
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                for _ in range(2):
-                    pos_dev.fill_(scratch_pos)
-                    step_dev.zero_()
-                    with ops.pdl(self.decode_pdl):
-                        self._decode_body(tok_dev, pos_dev, stage, log)
-            torch.cuda.current_stream().wait_stream(side)
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph), ops.pdl(self.decode_pdl):
-                logits = self._decode_body(tok_dev, pos_dev, stage, log)
-            self._decode_graph = (graph, tok_dev, pos_dev, logits, stage)
-            self._decode_log = log
-        _, tok_dev, pos_dev, _, _ = self._decode_graph
+        if sampling is None:
+            if self._decode_graph is None:
+                self._decode_graph = self._capture_decode(None)
+            self._armed = self._decode_graph
+        else:
+            if self._sample_params is None or self._sample_params.device != self.kv[0].device:
+                self._sample_params = torch.zeros((3,), device=self.kv[0].device, dtype=torch.int64)
+            self._sample_params.copy_(sampling)
+            if self._decode_graph_sampled is None:
+                self._decode_graph_sampled = self._capture_decode(self._sample_params)
+            self._armed = self._decode_graph_sampled
+        _, tok_dev, pos_dev, _, _ = self._armed
         tok_dev.fill_(int(first_token))
         pos_dev.fill_(self.kv_len)
         self._decode_log[1].zero_()
@@ -263,8 +295,8 @@ class DecoderEngine:
 
     def decode_graph_run(self, k: int) -> None:
         """Enqueue k token steps back to back (no host round trip in between: each replay embeds the token the previous one
-        left in device memory and logs its own arg-max into the device-side id buffer)."""
-        graph = self._decode_graph[0]
+        left in device memory and logs its own token into the device-side id buffer)."""
+        graph = self._armed[0]
         if self.kv_len + k > self.kv[0].shape[0]:
             raise RuntimeError(f"KV cache full ({self.kv_len} + {k} positions)")
         for _ in range(k):
@@ -278,14 +310,18 @@ class DecoderEngine:
         return self._decode_log[0][a:a + k].tolist()
 
     def decode_graph_step(self) -> torch.Tensor:
-        """Replay one token; returns the device int64[1] holding the NEW token (argmax), logits stay in the graph's
-        static buffer (`decode_graph_logits`)."""
-        graph, tok_dev, _, _, _ = self._decode_graph
+        """Replay one token; returns the device int64[1] holding the NEW token (the arg-max, or the draw when armed with
+        sampling); the greedy graph's logits stay in its static buffer (`decode_graph_logits`)."""
+        graph, tok_dev, _, _, _ = self._armed
         if self.kv_len >= self.kv[0].shape[0]:
             raise RuntimeError(f"KV cache full ({self.kv_len} positions)")
         graph.replay()
         self.kv_len += 1
         return tok_dev
+
+    def shared_seed(self, seed: int) -> int:
+        """The sampling seed every rank decoding this sequence uses (a single-GPU engine: its own)."""
+        return seed
 
     @property
     def decode_graph_logits(self) -> torch.Tensor:

@@ -149,6 +149,17 @@ class TPDecoderEngine(DecoderEngine):
         dist.all_gather(parts, local.contiguous(), group=self.group)
         return torch.cat(parts, dim=-1)
 
+    def shared_seed(self, seed: int) -> int:
+        """The first rank's sampling seed, on every rank of the group: the ranks then draw the same token from the identical
+        gathered logits, whatever state their own generators are in."""
+        if self.world == 1:
+            return seed
+        dev = self.device if dist.get_backend(self.group) == "nccl" else torch.device("cpu")
+        t = torch.tensor([seed], dtype=torch.int64, device=dev)
+        src = dist.get_global_rank(self.group, 0) if self.group is not None else 0
+        dist.broadcast(t, src=src, group=self.group)
+        return int(t.item())
+
     # ---- one layer -------------------------------------------------------------------------------------------------
     def _layer(self, L, x: torch.Tensor, S: int, pos0: int, qkv_out: Optional[torch.Tensor], ss_x: torch.Tensor):
         Hq, Hkv, D = self.Hq, self.Hkv, self.D

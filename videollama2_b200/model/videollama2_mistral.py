@@ -161,8 +161,10 @@ class Videollama2MistralForCausalLM(Videollama2MetaForCausalLM):
     # ---- generate (videollama2_mistral.py:110-144) -----------------------------------------------------------------
     @torch.no_grad()
     def generate(self, inputs=None, images=None, **kwargs):
-        """Greedy decoding, or sampling with HF's temperature / top-k(50) / top-p warpers when do_sample=True (optional
-        `generator=` for reproducibility); returns only the NEW token ids (as HF generate does with inputs_embeds)."""
+        """Greedy decoding, or sampling with HF's temperature / top-k(50) / top-p warpers when do_sample=True; returns only
+        the NEW token ids (as HF generate does with inputs_embeds).  Sampled tokens come from the vl2_sample_token kernel
+        on the device: the n-th new token is drawn with counter n from a seed taken once per call from `generator=`, or
+        from torch's default generator (torch.manual_seed makes runs reproducible)."""
         kwargs.pop("position_ids", None)
         attention_mask = kwargs.pop("attention_mask", None)
         if "inputs_embeds" in kwargs:
@@ -187,6 +189,18 @@ class Videollama2MistralForCausalLM(Videollama2MetaForCausalLM):
         else:
             inputs_embeds = self.get_model().embed_tokens(inputs)
         dec = self.get_model().decoder
+        params = None
+        if sample:        # one seed per call; a tensor-parallel decoder takes its first rank's
+            from ..sampling import draw_seed
+            params = ops.sampling_params(temperature, top_k, top_p, dec.shared_seed(draw_seed(rng)), dec.device)
+            counter = torch.zeros((1,), dtype=torch.int64, device=dec.device)
+            tok_out = torch.zeros((1,), dtype=torch.int64, device=dec.device)
+
+        def pick(logits, n: int) -> int:          # the n-th new token from its logits row
+            if params is None:
+                return int(torch.argmax(logits[0]).item())
+            return int(ops.sample_token(logits[0], params, counter, n, tok_out, dec.dtype).item())
+
         x = inputs_embeds[0].to(dec.dtype).contiguous()
         new_ids: List[int] = []
         # prefill once (keeps per-layer K/V), then one weight-streaming decode step per new token
@@ -194,27 +208,15 @@ class Videollama2MistralForCausalLM(Videollama2MetaForCausalLM):
         S = x.shape[0]
         self._cache_serial = getattr(self, "_cache_serial", 0) + 1        # handles of earlier forward(use_cache=True) calls die here
         logits, _ = dec.prefill(x, all_logits=False, keep_cache=use_cache and max_new > 1, max_len=S + max_new)
-        graphed = use_cache and max_new > 1 and dec.graph_decode
-        from ..sampling import sample_token
-        if graphed and not sample:
-            return self._generate_greedy_graphed(dec, logits, max_new, eos_ids, stopping, int(kwargs.get("decode_chunk", 8)))
+        if use_cache and max_new > 1 and dec.graph_decode:
+            return self._generate_graphed(dec, pick(logits, 0), max_new, eos_ids, stopping,
+                                          int(kwargs.get("decode_chunk", 8)), params)
         for step in range(max_new):
-            if sample:      # the graph's own argmax token is overridden below; its logits buffer is what we sample from
-                row = logits[0] if not (graphed and step > 0) else dec.decode_graph_logits[0]
-                tok = sample_token(row, temperature, top_p, top_k, rng)
-            else:
-                tok = int(torch.argmax(logits[0]).item()) if not (graphed and step > 0) else int(tok_dev.item())
+            tok = pick(logits, step)
             new_ids.append(tok)
             out_ids = torch.tensor([new_ids], dtype=torch.long)
             if tok in eos_ids or any(sc(out_ids, None) for sc in stopping) or step == max_new - 1:
                 break
-            if graphed:   # one graph launch per token: embed, 32 layers, lm_head, argmax all on the device
-                if step == 0:
-                    dec.decode_graph_begin(tok)
-                elif sample:
-                    tok_dev.fill_(tok)           # the replay embeds *tok_dev: the sampled token, not the argmax
-                tok_dev = dec.decode_graph_step()
-                continue
             e = self.get_model().embed_tokens(torch.tensor([tok]))
             if use_cache:
                 logits = dec.decode_step(e)
@@ -255,22 +257,23 @@ class Videollama2MistralForCausalLM(Videollama2MetaForCausalLM):
             res[b, : r.numel()] = r
         return res
 
-    def _generate_greedy_graphed(self, dec, logits, max_new: int, eos_ids, stopping, chunk: int):
-        """Greedy decoding with the host off the critical path: the captured single-token graph feeds itself (token and
-        position live in device memory) and appends every arg-max to a device-side id log, so the host enqueues `chunk`
-        replays at a time and reads the log once per chunk.  EOS / stopping criteria are evaluated on the host in token
-        order; tokens the device produced past the stopping point are discarded (at most chunk - 1 wasted steps), so the
-        returned ids equal the token-by-token loop's (tests/test_e2e_gpu.py)."""
+    def _generate_graphed(self, dec, first: int, max_new: int, eos_ids, stopping, chunk: int, sampling=None):
+        """Decoding with the host off the critical path: the captured single-token graph feeds itself (token and position
+        live in device memory) and appends every new token - the arg-max, or with `sampling` (an ops.sampling_params block)
+        the kernel's draw - to a device-side id log, so the host enqueues `chunk` replays at a time and reads the log once
+        per chunk.  `first` is new token 0, taken from the prefill logits.  EOS / stopping criteria are evaluated on the
+        host in token order; tokens the device produced past the stopping point are discarded (at most chunk - 1 wasted
+        steps), so the returned ids equal the token-by-token loop's (tests/test_e2e_gpu.py)."""
         ids_buf = torch.empty((1, max_new), dtype=torch.long)
 
         def stops(n):          # n = number of ids so far
             tok = int(ids_buf[0, n - 1])
             return tok in eos_ids or any(sc(ids_buf[:, :n], None) for sc in stopping) or n == max_new
 
-        ids_buf[0, 0] = int(torch.argmax(logits[0]).item())
+        ids_buf[0, 0] = first
         n = 1
         if not stops(n):
-            dec.decode_graph_begin(int(ids_buf[0, 0]))
+            dec.decode_graph_begin(first, sampling)
             done = False
             first = True
             while not done:

@@ -15,6 +15,7 @@ from ._lib import (ACT_GELU_ERF, ACT_GELU_TANH, ACT_NONE, ACT_QUICK_GELU, ACT_SI
 __all__ = [
     "gemm", "gemm_skinny", "attention", "attention_decode", "decode_rope_append", "attention_decode_dyn", "gemv", "decode_workspace", "l2_prefetch", "layernorm", "rmsnorm", "row_sumsq", "row_stats", "patch_im2col", "patch_embed", "clip_embed_finish",
     "dwconv3x3_ln_silu", "se_scale", "conv3d_im2col", "conv3d_k2s2", "rope_inplace", "embed_splice", "launch_count",
+    "sampling_params", "sample_token",
     "ACT_NONE", "ACT_QUICK_GELU", "ACT_SILU", "ACT_GELU_ERF", "ACT_GELU_TANH", "ACT_SWIGLU", "ACT_SIGMOID",
 ]
 
@@ -345,6 +346,37 @@ def attention_decode_dyn(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.
     check(_L(q).vl2_attention_decode_dyn(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), out.data_ptr(),
                                                k_cache.stride(0), pos_dev.data_ptr(), Hq, Hkv, D, float(scale),
                                                ws.data_ptr(), _stream()), "vl2_attention_decode_dyn")
+    return out
+
+
+def sampling_params(temperature: float, top_k: int, top_p: float, seed: int, device) -> torch.Tensor:
+    """The vl2_sample_params block of vl2_sample_token in device memory (int64 [3]); rejects the values
+    sampling.warp_logits rejects.  top_k = 0 (or >= V) turns top-k off, top_p = 1 turns top-p off."""
+    temperature, top_p, top_k = float(temperature), float(top_p), int(top_k)
+    if not (temperature > 0 and temperature != float("inf")):
+        raise ValueError(f"temperature must be positive and finite when sampling, got {temperature}")
+    if not (0.0 < top_p <= 1.0):
+        raise ValueError(f"top_p must lie in (0, 1], got {top_p}")
+    if top_k < 0:
+        raise ValueError(f"top_k must be >= 0, got {top_k}")
+    p = _lib.SampleParams(temperature=temperature, top_p=top_p, top_k=min(top_k, 2 ** 31 - 1), reserved=0,
+                          seed=int(seed) & (2 ** 64 - 1))
+    return torch.frombuffer(bytearray(bytes(p)), dtype=torch.int64).to(device)
+
+
+def sample_token(logits: torch.Tensor, params: torch.Tensor, counter_dev: torch.Tensor, counter_add: int,
+                 out: torch.Tensor, dtype: torch.dtype = torch.bfloat16) -> torch.Tensor:
+    """Draw one token id from the fp32 logits row [V] (or [1, V]) into out (int64 [1]) with counter *counter_dev +
+    counter_add; graph-capturable.  `dtype`: the model's storage type, which picks the library build (the kernel is the
+    same in both)."""
+    _need_cuda(logits, params, counter_dev, out)
+    assert logits.dtype == torch.float32 and logits.is_contiguous(), "sample_token: logits are one contiguous fp32 row"
+    assert params.dtype == torch.int64 and params.numel() == 3 and params.is_contiguous()
+    assert counter_dev.dtype == torch.int64 and counter_dev.numel() == 1
+    assert out.dtype == torch.int64 and out.numel() == 1
+    lib = _lib.load(dtype)
+    check(lib.vl2_sample_token(logits.data_ptr(), logits.numel(), params.data_ptr(), counter_dev.data_ptr(),
+                               int(counter_add), out.data_ptr(), _stream()), "vl2_sample_token", lib)
     return out
 
 
