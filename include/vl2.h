@@ -246,6 +246,39 @@ int vl2_sample_token(const float* logits, int V, const vl2_sample_params* params
                      int64_t counter_add, int64_t* token_out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Logits processors for generate(): HF's RepetitionPenaltyLogitsProcessor, NoRepeatNGramLogitsProcessor,
+ * NoBadWordsLogitsProcessor, MinNewTokensLengthLogitsProcessor and SuppressTokensLogitsProcessor (restated by
+ * videollama2_b200/sampling.py:process_logits), in place on one fp32 logits row [V], V <= 262144, one launch,
+ * graph-capturable.  The history is history[0 .. n), n = *n_dev + n_add: the ids generated so far.
+ *  - repetition_penalty p (1: off): every DISTINCT history token's score s becomes s < 0 ? s * p : s / p (fp32).
+ *  - no_repeat_ngram_size N (0: off): the last id of every N-gram of the history whose first N - 1 ids equal the history's
+ *    last N - 1 ids is banned.
+ *  - bad words: sequence q is bad_ids[bad_offsets[q] .. bad_offsets[q + 1]); one id is banned always, a longer sequence
+ *    of L ids bans its last id when n >= L and the history ends with its first L - 1 ids.
+ *  - every eos_ids entry is banned while n < min_new_tokens; every suppress_ids entry is banned always.
+ * Banned means -inf, after the penalty, whatever the score was.  Only listed indices are read or written; table entries
+ * outside [0, V) are skipped.  The block and its tables are read from device memory, so one captured graph serves every
+ * setting.
+ * ---------------------------------------------------------------------------------------------------------- */
+typedef struct vl2_logits_process_params {
+  float repetition_penalty;
+  int32_t no_repeat_ngram_size;
+  int64_t min_new_tokens;
+  int32_t n_eos;
+  int32_t n_suppress;
+  int32_t n_bad;
+  int32_t reserved;
+  const int64_t* eos_ids;        /* device [n_eos] */
+  const int64_t* suppress_ids;   /* device [n_suppress] */
+  const int64_t* bad_offsets;    /* device [n_bad + 1] */
+  const int64_t* bad_ids;        /* device [bad_offsets[n_bad]] */
+} vl2_logits_process_params;
+/* logits 4-byte aligned; params, history and n_dev 8-byte aligned and not null (VL2_E_BADALIGN); V outside
+ * [1, 262144]: VL2_E_BADSHAPE. */
+int vl2_process_logits(float* logits, int V, const vl2_logits_process_params* params, const int64_t* history,
+                       const int64_t* n_dev, int64_t n_add, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Row-wise normalisations (HBM-bound, one pass).
  * vl2_layernorm: y = act( LN(x; gamma, beta, eps) [+ residual] )  over the last dim C (bf16 in/out, fp32 math).
  *   act in {NONE, SILU}; with residual the order is act(LN(x) + residual)   (timm Bottleneck: act3(conv3(..)+shortcut)).

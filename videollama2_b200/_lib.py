@@ -18,7 +18,7 @@ SYMBOLS = [
     "vl2_patch_im2col", "vl2_clip_embed_finish",
     "vl2_dwconv3x3_ln_silu", "vl2_se_scale", "vl2_conv3d_im2col",
     "vl2_rope_inplace", "vl2_embed_splice", "vl2_tp_allreduce_stats", "vl2_patch_embed",
-    "vl2_sample_token",
+    "vl2_sample_token", "vl2_process_logits",
 ]
 
 ACT_NONE, ACT_QUICK_GELU, ACT_SILU, ACT_GELU_ERF, ACT_SWIGLU, ACT_GELU_TANH = 0, 1, 2, 3, 4, 5
@@ -74,6 +74,12 @@ class PatchEmbedArgs(C.Structure):
 class SampleParams(C.Structure):
     _fields_ = [("temperature", C.c_float), ("top_p", C.c_float), ("top_k", C.c_int32), ("reserved", C.c_int32),
                 ("seed", C.c_uint64)]
+
+
+class LogitsProcessParams(C.Structure):
+    _fields_ = [("repetition_penalty", C.c_float), ("no_repeat_ngram_size", C.c_int32), ("min_new_tokens", C.c_int64),
+                ("n_eos", C.c_int32), ("n_suppress", C.c_int32), ("n_bad", C.c_int32), ("reserved", C.c_int32),
+                ("eos_ids", C.c_void_p), ("suppress_ids", C.c_void_p), ("bad_offsets", C.c_void_p), ("bad_ids", C.c_void_p)]
 
 
 class Vl2Error(RuntimeError):
@@ -142,6 +148,7 @@ def load(dtype=None) -> C.CDLL:
         "vl2_tp_allreduce_stats": [C.POINTER(TpAllReduceArgs), vp],
         "vl2_patch_embed": [C.POINTER(PatchEmbedArgs), vp],
         "vl2_sample_token": [vp, i32, vp, vp, i64, vp, vp],
+        "vl2_process_logits": [vp, i32, vp, vp, vp, i64, vp],
     }
     for name, argtypes in sigs.items():
         fn = getattr(lib, name)

@@ -34,9 +34,14 @@ class DecoderEngine:
         self._graphed = None
         self._decode_graph = None   # (graph, tok_dev, pos_dev, logits, stage) of the captured greedy single-token step
         self._decode_graph_sampled = None   # the same step ending in vl2_sample_token instead of the arg-max
-        self._decode_bufs = None    # (tok_dev, pos_dev, stage, gen_buf, step_dev): device state both graphs share
+        # the greedy and sampled steps with vl2_process_logits in front of the token choice (captured on first use only)
+        self._decode_graph_processed = self._decode_graph_sampled_processed = None
+        self._decode_bufs = None    # (tok_dev, pos_dev, stage, gen_buf, step_dev): device state the graphs share
         self._decode_log = None     # (device id buffer, device step counter) the graphs append their tokens to
+        self._decode_hist = None    # new token 0 followed by the id log (gen_buf is its view from index 1)
         self._sample_params = None  # device vl2_sample_params the sampled graph reads (values copied in when armed)
+        self._process_params = None  # device vl2_logits_process_params block the processed graphs read (copied when armed)
+        self._process_tables = None  # the ops.logits_process_params tensor whose tables the armed block points into
         self._armed = None          # the graph decode_graph_begin armed last
         self._decode_read = 0
         self.graph_decode = False
@@ -55,8 +60,9 @@ class DecoderEngine:
         return self
 
     def _drop_decode_graphs(self) -> None:
-        """Forget both captured decode steps: they hold the addresses of the KV cache they were captured on."""
+        """Forget the captured decode steps: they hold the addresses of the KV cache they were captured on."""
         self._decode_graph = self._decode_graph_sampled = self._decode_bufs = self._armed = None
+        self._decode_graph_processed = self._decode_graph_sampled_processed = None
 
     def _prefill_last(self, embeds: torch.Tensor) -> torch.Tensor:
         return self.prefill(embeds, all_logits=False, keep_cache=False, _no_graph=True)[0]
@@ -195,12 +201,13 @@ class DecoderEngine:
 
     # ---- the same step as ONE CUDA graph ---------------------------------------------------------------------
     def _decode_body(self, tok_dev: torch.Tensor, pos_dev: torch.Tensor, stage: torch.Tensor, log=None,
-                     sampler: Optional[torch.Tensor] = None) -> torch.Tensor:
+                     sampler: Optional[torch.Tensor] = None, processor: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Single-token step whose position and token live in device memory: embeds *tok_dev, appends K/V at *pos_dev,
         writes argmax(logits) back to tok_dev and increments pos_dev, so one captured graph serves every token.
         `sampler` (a device vl2_sample_params block, needs `log`): the new token is drawn by vl2_sample_token with
         counter *step_dev + 1 instead - the n-th new token of a generate() call uses counter n, token 0 came from the
-        prefill."""
+        prefill.  `processor` (a device vl2_logits_process_params block, needs `log`): vl2_process_logits edits the
+        logits first, with the history _decode_hist[0 .. *step_dev + 1) = new tokens 0 .. n - 1."""
         Hq, Hkv, D = self.Hq, self.Hkv, self.D
         x = torch.index_select(self.w["embed"], 0, tok_dev)
         o = torch.empty((1, Hq * D), device=x.device, dtype=self.dtype)
@@ -232,6 +239,8 @@ class DecoderEngine:
             h = ops.gemv(x, L["wgu"], act=ops.ACT_SWIGLU, rms_eps=self.eps)
             x = ops.gemv(h, L["wd"], residual=x)
         logits = ops.gemv(x, self.w["lm_head"], rms_eps=self.eps, out_dtype=torch.float32)
+        if processor is not None:
+            ops.process_logits(logits, processor, self._decode_hist, log[1], 1, self.dtype)
         if sampler is None:
             tok_dev.copy_(torch.argmax(logits, dim=1))
         else:
@@ -243,14 +252,16 @@ class DecoderEngine:
             step_dev.add_(1)
         return logits
 
-    def _capture_decode(self, sampler: Optional[torch.Tensor]):
-        """Capture the single-token step (greedy, or sampled with the parameter block `sampler`) on the shared buffers."""
+    def _capture_decode(self, sampler: Optional[torch.Tensor], processor: Optional[torch.Tensor] = None):
+        """Capture the single-token step (greedy, or sampled with the parameter block `sampler`; with the processor
+        block `processor`, the logits processors first) on the shared buffers."""
         dev = self.kv[0].device
         if self._decode_bufs is None:
+            self._decode_hist = torch.zeros((self.kv[0].shape[0] + 2,), device=dev, dtype=torch.int64)
             self._decode_bufs = (torch.zeros((1,), device=dev, dtype=torch.int64),
                                  torch.zeros((1,), device=dev, dtype=torch.int32),
                                  torch.empty((1, (self.Hq + 2 * self.Hkv) * self.D), device=dev, dtype=self.dtype),
-                                 torch.zeros((self.kv[0].shape[0] + 1,), device=dev, dtype=torch.int64),
+                                 self._decode_hist[1:],
                                  torch.zeros((1,), device=dev, dtype=torch.int64))
             self._decode_log = self._decode_bufs[3:]
         tok_dev, pos_dev, stage, _, step_dev = self._decode_bufs
@@ -263,32 +274,53 @@ class DecoderEngine:
                 pos_dev.fill_(scratch_pos)
                 step_dev.zero_()
                 with ops.pdl(self.decode_pdl):
-                    self._decode_body(tok_dev, pos_dev, stage, log, sampler)
+                    self._decode_body(tok_dev, pos_dev, stage, log, sampler, processor)
         torch.cuda.current_stream().wait_stream(side)
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph), ops.pdl(self.decode_pdl):
-            logits = self._decode_body(tok_dev, pos_dev, stage, log, sampler)
+            logits = self._decode_body(tok_dev, pos_dev, stage, log, sampler, processor)
         return (graph, tok_dev, pos_dev, logits, stage)
 
-    def decode_graph_begin(self, first_token: int, sampling: Optional[torch.Tensor] = None) -> None:
+    def decode_graph_begin(self, first_token: int, sampling: Optional[torch.Tensor] = None,
+                           processing: Optional[torch.Tensor] = None) -> None:
         """Arm the graph-replayed decode loop after prefill(keep_cache=True): token := first_token, pos := kv_len.
         `sampling`: an ops.sampling_params block - arm the sampled graph (captured once, then reused for every parameter
-        setting) instead of the greedy one."""
+        setting) instead of the greedy one.  `processing`: an ops.logits_process_params tensor - arm the variant of that
+        graph with the logits processors (also captured once; the tensor is kept alive while armed)."""
         if not self.kv:
             raise RuntimeError("decode_graph_begin needs prefill(keep_cache=True) first")
+        dev = self.kv[0].device
+        proc = None
+        if processing is not None:
+            if self._process_params is None or self._process_params.device != dev:
+                self._process_params = torch.zeros((ops.PROCESS_HEADER_WORDS,), device=dev, dtype=torch.int64)
+            self._process_params.copy_(processing[:ops.PROCESS_HEADER_WORDS])
+            self._process_tables = processing
+            proc = self._process_params
         if sampling is None:
-            if self._decode_graph is None:
-                self._decode_graph = self._capture_decode(None)
-            self._armed = self._decode_graph
+            if proc is None:
+                if self._decode_graph is None:
+                    self._decode_graph = self._capture_decode(None)
+                self._armed = self._decode_graph
+            else:
+                if self._decode_graph_processed is None:
+                    self._decode_graph_processed = self._capture_decode(None, proc)
+                self._armed = self._decode_graph_processed
         else:
-            if self._sample_params is None or self._sample_params.device != self.kv[0].device:
-                self._sample_params = torch.zeros((3,), device=self.kv[0].device, dtype=torch.int64)
+            if self._sample_params is None or self._sample_params.device != dev:
+                self._sample_params = torch.zeros((3,), device=dev, dtype=torch.int64)
             self._sample_params.copy_(sampling)
-            if self._decode_graph_sampled is None:
-                self._decode_graph_sampled = self._capture_decode(self._sample_params)
-            self._armed = self._decode_graph_sampled
+            if proc is None:
+                if self._decode_graph_sampled is None:
+                    self._decode_graph_sampled = self._capture_decode(self._sample_params)
+                self._armed = self._decode_graph_sampled
+            else:
+                if self._decode_graph_sampled_processed is None:
+                    self._decode_graph_sampled_processed = self._capture_decode(self._sample_params, proc)
+                self._armed = self._decode_graph_sampled_processed
         _, tok_dev, pos_dev, _, _ = self._armed
         tok_dev.fill_(int(first_token))
+        self._decode_hist[0].fill_(int(first_token))
         pos_dev.fill_(self.kv_len)
         self._decode_log[1].zero_()
         self._decode_read = 0

@@ -164,7 +164,12 @@ class Videollama2MistralForCausalLM(Videollama2MetaForCausalLM):
         """Greedy decoding, or sampling with HF's temperature / top-k(50) / top-p warpers when do_sample=True; returns only
         the NEW token ids (as HF generate does with inputs_embeds).  Sampled tokens come from the vl2_sample_token kernel
         on the device: the n-th new token is drawn with counter n from a seed taken once per call from `generator=`, or
-        from torch's default generator (torch.manual_seed makes runs reproducible)."""
+        from torch's default generator (torch.manual_seed makes runs reproducible).
+        HF's logits processors run before the token choice on every decode path, on the device (vl2_process_logits):
+        repetition_penalty, no_repeat_ngram_size, min_new_tokens / min_length, bad_words_ids and suppress_tokens, with the
+        semantics of transformers 5.5's generate(inputs_embeds=...) - the history is the new tokens only, min_length
+        counts the spliced prompt (sampling.generate_processors; the same arithmetic in the reference's pinned 4.40 is
+        unverified).  Without them generation is unchanged."""
         kwargs.pop("position_ids", None)
         attention_mask = kwargs.pop("attention_mask", None)
         if "inputs_embeds" in kwargs:
@@ -196,21 +201,34 @@ class Videollama2MistralForCausalLM(Videollama2MetaForCausalLM):
             counter = torch.zeros((1,), dtype=torch.int64, device=dec.device)
             tok_out = torch.zeros((1,), dtype=torch.int64, device=dec.device)
 
-        def pick(logits, n: int) -> int:          # the n-th new token from its logits row
-            if params is None:
-                return int(torch.argmax(logits[0]).item())
-            return int(ops.sample_token(logits[0], params, counter, n, tok_out, dec.dtype).item())
-
         x = inputs_embeds[0].to(dec.dtype).contiguous()
+        S = x.shape[0]
+        from ..sampling import generate_processors
+        proc = generate_processors(kwargs, eos_ids, S, self.vocab_size)
+        if proc is not None:      # every rank of a tensor-parallel decoder builds the same tables from the same kwargs
+            proc = ops.logits_process_params(self.vocab_size, dec.device, **proc)
+            history = torch.zeros((max(max_new, 1),), dtype=torch.int64, device=dec.device)
+            zero = torch.zeros((1,), dtype=torch.int64, device=dec.device)
+
+        def pick(logits, n: int) -> int:          # the n-th new token from its logits row
+            if proc is not None:                  # processors first, on the ids new tokens 0 .. n - 1
+                ops.process_logits(logits[0], proc, history, zero, n, dec.dtype)
+            if params is None:
+                tok = int(torch.argmax(logits[0]).item())
+            else:
+                tok = int(ops.sample_token(logits[0], params, counter, n, tok_out, dec.dtype).item())
+            if proc is not None and n < max_new:
+                history[n] = tok
+            return tok
+
         new_ids: List[int] = []
         # prefill once (keeps per-layer K/V), then one weight-streaming decode step per new token
         use_cache = kwargs.get("use_cache", True)
-        S = x.shape[0]
         self._cache_serial = getattr(self, "_cache_serial", 0) + 1        # handles of earlier forward(use_cache=True) calls die here
         logits, _ = dec.prefill(x, all_logits=False, keep_cache=use_cache and max_new > 1, max_len=S + max_new)
         if use_cache and max_new > 1 and dec.graph_decode:
             return self._generate_graphed(dec, pick(logits, 0), max_new, eos_ids, stopping,
-                                          int(kwargs.get("decode_chunk", 8)), params)
+                                          int(kwargs.get("decode_chunk", 8)), params, proc)
         for step in range(max_new):
             tok = pick(logits, step)
             new_ids.append(tok)
@@ -229,7 +247,9 @@ class Videollama2MistralForCausalLM(Videollama2MetaForCausalLM):
         """Batch > 1 (HF `generate` semantics of videollama2_mistral.py:110-144 for a padded batch): the rows are decoded
         one after the other through the batch-1 path - each row keeps its own real tokens (`attention_mask`), takes the
         images its placeholders consume in order (a row without a placeholder consumes one slot, videollama2_arch.py:181-191)
-        - and the new ids are right-padded with `pad_token_id` to the longest row, as HF pads finished sequences."""
+        - and the new ids are right-padded with `pad_token_id` to the longest row, as HF pads finished sequences.  Logits
+        processors run per row on that row's new ids; `min_length` counts the row's own spliced length, where HF counts the
+        batch's padded length."""
         from ..mm_utils import splice_plan
         if kwargs.get("stopping_criteria"):
             raise NotImplementedError("stopping_criteria with batch > 1 (the criteria objects are built for one prompt)")
@@ -257,10 +277,12 @@ class Videollama2MistralForCausalLM(Videollama2MetaForCausalLM):
             res[b, : r.numel()] = r
         return res
 
-    def _generate_graphed(self, dec, first: int, max_new: int, eos_ids, stopping, chunk: int, sampling=None):
+    def _generate_graphed(self, dec, first: int, max_new: int, eos_ids, stopping, chunk: int, sampling=None,
+                          processing=None):
         """Decoding with the host off the critical path: the captured single-token graph feeds itself (token and position
         live in device memory) and appends every new token - the arg-max, or with `sampling` (an ops.sampling_params block)
-        the kernel's draw - to a device-side id log, so the host enqueues `chunk` replays at a time and reads the log once
+        the kernel's draw, after the logits processors of `processing` (an ops.logits_process_params tensor) when given -
+        to a device-side id log, so the host enqueues `chunk` replays at a time and reads the log once
         per chunk.  `first` is new token 0, taken from the prefill logits.  EOS / stopping criteria are evaluated on the
         host in token order; tokens the device produced past the stopping point are discarded (at most chunk - 1 wasted
         steps), so the returned ids equal the token-by-token loop's (tests/test_e2e_gpu.py)."""
@@ -273,7 +295,7 @@ class Videollama2MistralForCausalLM(Videollama2MetaForCausalLM):
         ids_buf[0, 0] = first
         n = 1
         if not stops(n):
-            dec.decode_graph_begin(first, sampling)
+            dec.decode_graph_begin(first, sampling, processing)
             done = False
             first = True
             while not done:

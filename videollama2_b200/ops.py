@@ -15,7 +15,7 @@ from ._lib import (ACT_GELU_ERF, ACT_GELU_TANH, ACT_NONE, ACT_QUICK_GELU, ACT_SI
 __all__ = [
     "gemm", "gemm_skinny", "attention", "attention_decode", "decode_rope_append", "attention_decode_dyn", "gemv", "decode_workspace", "l2_prefetch", "layernorm", "rmsnorm", "row_sumsq", "row_stats", "patch_im2col", "patch_embed", "clip_embed_finish",
     "dwconv3x3_ln_silu", "se_scale", "conv3d_im2col", "conv3d_k2s2", "rope_inplace", "embed_splice", "launch_count",
-    "sampling_params", "sample_token",
+    "sampling_params", "sample_token", "logits_process_params", "process_logits",
     "ACT_NONE", "ACT_QUICK_GELU", "ACT_SILU", "ACT_GELU_ERF", "ACT_GELU_TANH", "ACT_SWIGLU", "ACT_SIGMOID",
 ]
 
@@ -378,6 +378,54 @@ def sample_token(logits: torch.Tensor, params: torch.Tensor, counter_dev: torch.
     check(lib.vl2_sample_token(logits.data_ptr(), logits.numel(), params.data_ptr(), counter_dev.data_ptr(),
                                int(counter_add), out.data_ptr(), _stream()), "vl2_sample_token", lib)
     return out
+
+
+PROCESS_HEADER_WORDS = C.sizeof(_lib.LogitsProcessParams) // 8     # the vl2_logits_process_params block, in int64 words
+
+
+def logits_process_params(V: int, device, repetition_penalty=None, no_repeat_ngram_size=None, min_new_tokens: int = 0,
+                          eos_token_ids=(), bad_words_ids=None, suppress_tokens=None) -> torch.Tensor:
+    """The vl2_logits_process_params block of vl2_process_logits and its tables in one device int64 tensor: the block is
+    the first PROCESS_HEADER_WORDS words, its table pointers point into the rest.  The settings and their validation are
+    sampling.check_processors' (ValueError for what HF's processors reject and for ids outside [0, V)).  The block may be
+    copied elsewhere (a captured graph's fixed block) while this tensor stays alive."""
+    from .sampling import check_processors
+    cfg = check_processors(V, repetition_penalty, no_repeat_ngram_size, min_new_tokens, eos_token_ids, bad_words_ids,
+                           suppress_tokens)
+    bad = cfg["bad_words_ids"] or ()
+    offsets = [0]
+    for s in bad:
+        offsets.append(offsets[-1] + len(s))
+    tables = [list(cfg["eos_token_ids"]), list(cfg["suppress_tokens"]), offsets, [t for s in bad for t in s]]
+    buf = torch.empty((PROCESS_HEADER_WORDS + sum(len(t) for t in tables),), dtype=torch.int64, device=device)
+    addr, ptrs = buf.data_ptr() + 8 * PROCESS_HEADER_WORDS, []
+    for t in tables:
+        ptrs.append(addr)
+        addr += 8 * len(t)
+    hdr = _lib.LogitsProcessParams(
+        repetition_penalty=cfg["repetition_penalty"] or 1.0, no_repeat_ngram_size=cfg["no_repeat_ngram_size"] or 0,
+        min_new_tokens=cfg["min_new_tokens"], n_eos=len(tables[0]), n_suppress=len(tables[1]), n_bad=len(bad),
+        reserved=0, eos_ids=ptrs[0], suppress_ids=ptrs[1], bad_offsets=ptrs[2], bad_ids=ptrs[3])
+    host = torch.cat([torch.frombuffer(bytearray(bytes(hdr)), dtype=torch.int64),
+                      torch.tensor([x for t in tables for x in t], dtype=torch.int64)])
+    buf.copy_(host)
+    return buf
+
+
+def process_logits(logits: torch.Tensor, params: torch.Tensor, history: torch.Tensor, n_dev: torch.Tensor, n_add: int,
+                   dtype: torch.dtype = torch.bfloat16) -> torch.Tensor:
+    """Apply the logits processors of `params` (logits_process_params' tensor, or a copy of its block) in place to the
+    fp32 logits row [V] (or [1, V]) after the generated ids history[0 .. *n_dev + n_add); graph-capturable.  `dtype`:
+    the model's storage type, which picks the library build (the kernel is the same in both)."""
+    _need_cuda(logits, params, history, n_dev)
+    assert logits.dtype == torch.float32 and logits.is_contiguous(), "process_logits: logits are one contiguous fp32 row"
+    assert params.dtype == torch.int64 and params.numel() >= PROCESS_HEADER_WORDS and params.is_contiguous()
+    assert history.dtype == torch.int64 and history.is_contiguous()
+    assert n_dev.dtype == torch.int64 and n_dev.numel() == 1
+    lib = _lib.load(dtype)
+    check(lib.vl2_process_logits(logits.data_ptr(), logits.numel(), params.data_ptr(), history.data_ptr(),
+                                 n_dev.data_ptr(), int(n_add), _stream()), "vl2_process_logits", lib)
+    return logits
 
 
 def layernorm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: float, *, act: int = ACT_NONE,
