@@ -56,9 +56,11 @@ const char* vl2_last_error(void);
 int64_t vl2_launch_count(void);
 /* Programmatic dependent launch for every subsequent vl2_* launch of this process: 1 = on (each kernel is launched with
  * the programmatic-stream-serialization attribute; kernels begin with griddepcontrol.launch_dependents and wait with
- * griddepcontrol.wait before touching their inputs, so a kernel's prologue - for the GEMV: the first weight-stage
- * prefetches - overlaps the tail of its predecessor), 0 = off, -1 = follow the VL2_PDL environment variable (default off).
- * Used by the single-token decode graph, where ~230 small kernels run back to back. */
+ * griddepcontrol.wait before touching global memory, so a kernel's prologue overlaps the tail of its predecessor),
+ * 0 = off, -1 = follow the VL2_PDL environment variable (default off).  Used by the single-token decode graph, where ~230
+ * small kernels run back to back.  Before its wait a kernel touches no global memory, with two exceptions: the GEMV
+ * (vl2_gemv_bf16) bulk-loads its first weight stages of W, and the L2 prefetch (vl2_l2_prefetch) does not wait at all,
+ * since it moves no data.  So under PDL the launch right before a GEMV must not write that GEMV's W. */
 int vl2_set_pdl(int mode);
 
 /* ------------------------------------------------------------------------------------------------------------
@@ -171,7 +173,10 @@ int vl2_gemm_skinny(const void* A, int a_f32, const void* W, const float* bias, 
 /* GEMV, the M = 1 case of the above as its own entry point (every nn.Linear of a single-token decode step):
  * y[N] = act(s * W[N,K] x + bias) (+ residual); with rms_eps > 0, s = rsqrt(mean(x^2) + rms_eps): the RMSNorm in front of
  * the projection (HF:mistral/modeling_mistral.py:35-48) with its gain folded into W's columns, at no extra pass over x.
- * act as vl2_gemm_skinny.  HBM-bound: 2*N*K bytes. */
+ * act as vl2_gemm_skinny.  HBM-bound: 2*N*K bytes.
+ * Under programmatic dependent launch (vl2_set_pdl) the first stages of W are loaded before griddepcontrol.wait, while
+ * the producer of x drains: W is a constant that the launch just before this one must not write.  Everything else (x,
+ * bias, residual, y) is touched only after the wait.  The dependents are released after the k-loop, before the stores. */
 int vl2_gemv_bf16(const void* x, const void* W, const float* bias, const void* residual /* bf16 [N] or NULL */, void* y,
                   int out_f32, int N, int K, int act, float rms_eps, void* stream);
 

@@ -87,6 +87,19 @@ class Vl2Error(RuntimeError):
 
 
 _libs = {}
+# programmatic dependent launch mode of every loaded build (vl2_set_pdl): -1 = follow VL2_PDL, 0 = off, 1 = on.
+# ops.pdl sets it; a build loaded later starts in the same mode.
+pdl_mode = -1
+
+
+def set_pdl(mode: int) -> None:
+    """Switch every loaded build, and every build loaded later, to PDL mode `mode` (-1, 0 or 1)."""
+    global pdl_mode
+    if mode not in (-1, 0, 1):
+        raise ValueError(f"PDL mode must be -1, 0 or 1, not {mode}")
+    pdl_mode = mode
+    for lib in _libs.values():
+        check(lib.vl2_set_pdl(mode), "vl2_set_pdl", lib)
 
 
 def _variant(dtype) -> str:
@@ -157,6 +170,7 @@ def load(dtype=None) -> C.CDLL:
     lib.vl2_storage_dtype.restype = C.c_int
     if int(lib.vl2_storage_dtype()) != (0 if var == "bf16" else 1):
         raise Vl2Error(f"{path} was built for the other storage type")
+    check(lib.vl2_set_pdl(pdl_mode), "vl2_set_pdl", lib)
     _libs[var] = lib
     return lib
 

@@ -25,6 +25,7 @@ resample_h_kernel(const uint8_t* __restrict__ src, uint8_t* __restrict__ tmp, in
                   int off_y, int off_x, uint32_t pad_rgb, int out_w, const int* __restrict__ bounds,
                   const int* __restrict__ kk, int ksize) {
   extern __shared__ uint8_t row[];   // [canvas_w * 3]
+  pdl_wait();   // under PDL the producer of the frames may still be running, or still reading what tmp overwrites
   const int cy = blockIdx.x, t = blockIdx.y;
   const int iy = cy - off_y;
   const uint8_t pr = pad_rgb & 0xff, pg = (pad_rgb >> 8) & 0xff, pb = (pad_rgb >> 16) & 0xff;
@@ -61,6 +62,7 @@ __global__ void __launch_bounds__(128)
 resample_v_kernel(const uint8_t* __restrict__ tmp, __nv_bfloat16* __restrict__ out, uint8_t* __restrict__ out_u8,
                   int canvas_h, int out_w, int crop_top, int crop_left, int crop, const int* __restrict__ bounds,
                   const int* __restrict__ kk, int ksize, const float* __restrict__ lut) {
+  pdl_wait();   // tmp is resample_h's output, and the kernels after this one wait only for this grid
   const int x = blockIdx.x * blockDim.x + threadIdx.x;   // column inside the crop window
   const int y = blockIdx.y, t = blockIdx.z;
   if (x >= crop) return;

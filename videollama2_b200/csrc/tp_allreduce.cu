@@ -67,7 +67,10 @@ tp_allreduce_stats_kernel(const TpArParams p) {
   __shared__ float red[64];
   const int tid = threadIdx.x;
   uint32_t* my_pad = p.pads[p.rank];
-  // ---- start barrier: every rank's partial is complete (its producing GEMM precedes this kernel in its stream)
+  // the producing GEMM / GEMV precedes this kernel in its stream, but under PDL it triggers before its stores: wait for
+  // it before signalling that this rank's partial is complete
+  pdl_wait();
+  // ---- start barrier: every rank's partial is complete
   if (blockIdx.x == 0 && tid < p.world) signal_add_sys(p.pads[tid] + p.rank);
   if (tid < p.world) wait_ge(my_pad + tid, p.epoch);
   __syncthreads();

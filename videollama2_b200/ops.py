@@ -228,20 +228,21 @@ def gemm_skinny(a: torch.Tensor, w: torch.Tensor, *, bias: Optional[torch.Tensor
 
 
 class pdl:
-    """Context manager: programmatic dependent launch for the vl2 launches inside (vl2_set_pdl)."""
+    """Context manager: programmatic dependent launch on or off for the vl2 launches inside (vl2_set_pdl), in both
+    builds, including one first loaded inside the block.  Blocks nest: on exit the enclosing block's mode (or, outside
+    every block, the VL2_PDL environment variable) applies again."""
 
     def __init__(self, on: bool = True):
         self.on = on
+        self._outer = []
 
     def __enter__(self):
-        _lib.load()
-        for lib in _lib._libs.values():
-            check(lib.vl2_set_pdl(1 if self.on else 0), "vl2_set_pdl")
+        self._outer.append(_lib.pdl_mode)
+        _lib.set_pdl(1 if self.on else 0)
         return self
 
     def __exit__(self, *exc):
-        for lib in _lib._libs.values():
-            check(lib.vl2_set_pdl(-1), "vl2_set_pdl")
+        _lib.set_pdl(self._outer.pop())
         return False
 
 
