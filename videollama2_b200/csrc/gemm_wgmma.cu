@@ -1,16 +1,21 @@
 // Persistent warp-specialised bf16 GEMM for sm_90a:  C[M,Nout] = epi(A[M,K] * W[N,K]^T).
 //
-//   warpgroup 0   TMA producer (one thread): cp.async.bulk.tensor A/B tiles -> 128B-swizzled smem ring
+//   warpgroup 0   TMA producer (one thread): cp.async.bulk.tensor A/B tiles -> 128B-swizzled smem ring;
+//                 epilogue operands (epilogue variants only), during the k-loop: warp 1 loads the tile's residual /
+//                 RoPE-table slots by TMA into a small smem ring, warps 2-3 compute its 128 row factors into smem
 //   warpgroups 1, 2  consumers: wgmma.mma_async m64 x BN x k16 from the ring (rows 0..63 / 64..127 of the 128-row tile),
-//                 fp32 accumulators in registers, then the epilogue straight from the accumulator fragments:
-//                 row_scale / folded RMSNorm or LayerNorm / bias / activation / SwiGLU / RoPE / residual / statistics
-//                 -> global (optionally also to peer buffers or an NVSwitch multicast address)
+//                 fp32 accumulators in registers, then the epilogue from the accumulator fragments:
+//                 row_scale / folded RMSNorm or LayerNorm / bias / activation / SwiGLU / RoPE / residual / statistics.
+//                 A variant writes each 16 x 32 slot of a warp into a swizzled smem staging tile that one lane stores by
+//                 TMA; the generic epilogue stores to global directly (optionally also to peer buffers or an NVSwitch
+//                 multicast address)
 //
 // Tiles are 128 x BN, BN in {64,...,256} step 32 chosen per launch by a wave / operand-traffic cost model (choose_tile);
 // BLOCK_K = 64 bf16 = one 128-byte swizzle atom; the grid is persistent (<= #SMs CTAs, static round-robin over tiles,
-// M fastest so that a wave shares W tiles through L2).  M/N/K tails: TMA zero-fills out-of-bounds reads, stores are
-// predicated.
+// M fastest so that a wave shares W tiles through L2).  M/N/K tails: TMA zero-fills out-of-bounds reads; TMA stores clip
+// at the output's bounds, the generic epilogue's stores are predicated.
 #include <stdlib.h>
+#include <string.h>
 
 #include "host_common.h"
 #include "ptx.cuh"
@@ -22,6 +27,18 @@ static constexpr int BK = 64;
 static constexpr int kConsumerThreads = 256;              // two consumer warpgroups
 static constexpr int kGemmThreads = 128 + kConsumerThreads;
 static constexpr int kConvLine = 16;                      // Conv3d front end: output lines and columns per time step are padded to 16
+
+// Shared memory of the epilogue variants, carved out of the 227 KB next to the A/B ring:
+//   output staging: per consumer warp two 16-row x 32-column 16-bit tiles (64-byte rows, SWIZZLE_64B; SwiGLU: 16 columns,
+//                   32-byte rows, SWIZZLE_32B), each written by the warp and stored by one TMA store;
+//   operand ring:   kOpSlots 128-row x 32-column slots of the residual or of the RoPE table (64-byte rows, SWIZZLE_64B);
+//   row factors:    the tile's 128 row factors, double-buffered (tile t / t + 1).
+static constexpr int kOpSlots = 2;
+static constexpr int kOpSlotBytes = 128 * 64;
+static constexpr int kStageTileBytes = 16 * 64;
+static constexpr int kEpiOutBytes = (kConsumerThreads / 32) * 2 * kStageTileBytes;
+static constexpr int kEpiSmemBytes = kEpiOutBytes + kOpSlots * kOpSlotBytes + 2 * 128 * 4;
+static constexpr int kSmemLimit = 227 * 1024;
 
 // PAIR = true: the two CTAs of a cluster compute a 256 x BN tile (128 rows each) and share its B tile: each CTA loads
 // HALF of the B rows and the TMA unit multicasts them into both CTAs' shared memory, so a k-block costs
@@ -36,9 +53,10 @@ struct GemmCfg {
   static constexpr int kHalfBytesB = BN / 2 * BK * 2;     // pair: the half of B one CTA loads (1024-byte multiple)
   static constexpr int kStageBytes = kStageBytesA + kStageBytesB;
   static constexpr int kExtraBytes = 1024;               // barriers
-  static constexpr int kMaxStages = (227 * 1024 - kExtraBytes) / kStageBytes;
+  static constexpr int kMaxStages = (kSmemLimit - kExtraBytes - kEpiSmemBytes) / kStageBytes;
   static constexpr int kStages = kMaxStages > 8 ? 8 : kMaxStages;
-  static constexpr int kSmemBytes = kStages * kStageBytes + kExtraBytes;
+  static_assert(kStages >= 4, "the ring must keep at least 4 stages next to the epilogue's shared memory");
+  static constexpr int kSmemBytes = kStages * kStageBytes + kEpiSmemBytes + kExtraBytes;
   static constexpr int kAcc = BN / 2;                     // fp32 accumulators per consumer thread
   static constexpr int kEmptyArrivals = (PAIR ? 2 : 1) * (kConsumerThreads / 32);
   static_assert(!PAIR || kHalfBytesB % 1024 == 0, "the peer's half of B must start on a swizzle-atom boundary");
@@ -84,9 +102,9 @@ struct GemmParams {
 };
 
 // [0] items traced; per item t (<= 7), at 8*t + 4: consumer starts the item, 8*t + 5: accumulator complete,
-// 8*t + 6: its part of the tile is stored.  Inside the item's first 32-column slot (generic epilogue): 8*t + 1: its
-// accumulators selected, 8*t + 2: its residuals loaded (both -1 in a variant), 8*t + 3: the slot stored (every epilogue);
-// 8*t + 7 is scratch.
+// 8*t + 6: its part of the tile is stored (a variant: its last TMA store issued and done reading shared memory).  Inside
+// the item's first 32-column slot (generic epilogue): 8*t + 1: its accumulators selected, 8*t + 2: its residuals loaded
+// (both -1 in a variant), 8*t + 3: the slot stored (every epilogue; a variant: its TMA store issued); 8*t + 7 is scratch.
 __device__ long long g_gemm_trace[128];
 
 // one 4-byte store replicated by the NVSwitch to every GPU of the multicast group
@@ -151,14 +169,24 @@ __device__ __forceinline__ void release_slot(uint64_t* empty_bar, uint32_t rank)
 
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory"); }
 
-// sum the producer's per-32-column partials of one row in a fixed order (deterministic: no atomics anywhere)
+// sum the producer's per-32-column partials of one row in a fixed order (deterministic: no atomics anywhere).  kRolled
+// keeps the vector loop rolled (the same sums in the same order): for the row-factor warps, which run with 40 registers.
+template <bool kRolled>
 __device__ __forceinline__ float sum_parts(const float* pp, int nparts) {
   const int nvec = (nparts % 4 == 0) ? nparts : 0;   // rows are 16-byte aligned only then
   float q = 0.f;
   int i = 0;
-  for (; i + 4 <= nvec; i += 4) {
-    const float4 t4 = *reinterpret_cast<const float4*>(pp + i);
-    q += (t4.x + t4.y) + (t4.z + t4.w);
+  if (kRolled) {
+#pragma unroll 1
+    for (; i + 4 <= nvec; i += 4) {
+      const float4 t4 = *reinterpret_cast<const float4*>(pp + i);
+      q += (t4.x + t4.y) + (t4.z + t4.w);
+    }
+  } else {
+    for (; i + 4 <= nvec; i += 4) {
+      const float4 t4 = *reinterpret_cast<const float4*>(pp + i);
+      q += (t4.x + t4.y) + (t4.z + t4.w);
+    }
   }
   for (; i < nparts; ++i) q += pp[i];
   return q;
@@ -179,23 +207,30 @@ struct EpiRows {
   float mu[2];    // folded LayerNorm mean
   bool ok[2];
 };
+// The row factor of output row `row` (1 past p.M) and its folded LayerNorm mean (0 without).  The consumers of the generic
+// epilogue compute it for their own rows; for a variant the epilogue-operand warp computes the tile's rows into shared
+// memory during the k-loop.
+template <bool kRolled>
+__device__ __forceinline__ float row_factor(const GemmParams& p, int row, float& mu) {
+  float rs = (p.row_scale != nullptr && row < p.M) ? p.row_scale[row] : 1.f;
+  mu = 0.f;
+  if (p.rms_sumsq_in != nullptr && row < p.M) {
+    float q = sum_parts<kRolled>(p.rms_sumsq_in + (int64_t)row * p.rms_nparts, p.rms_nparts) * p.rms_inv_dim;   // E[x^2]
+    if (p.ln_sum_in != nullptr) {
+      mu = sum_parts<kRolled>(p.ln_sum_in + (int64_t)row * p.rms_nparts, p.rms_nparts) * p.rms_inv_dim;
+      q = fmaxf(q - mu * mu, 0.f);                                                                      // variance
+    }
+    rs *= rsqrtf(q + p.rms_eps);
+  }
+  return rs;
+}
 __device__ __forceinline__ EpiRows epi_rows(const GemmParams& p, int m0, int rloc) {
   EpiRows r;
-  const bool ln = p.ln_sum_in != nullptr;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int row = m0 + rloc + 8 * h;
     r.ok[h] = row < p.M;
-    r.rs[h] = (p.row_scale != nullptr && r.ok[h]) ? p.row_scale[row] : 1.f;
-    r.mu[h] = 0.f;
-    if (p.rms_sumsq_in != nullptr && r.ok[h]) {
-      float q = sum_parts(p.rms_sumsq_in + (int64_t)row * p.rms_nparts, p.rms_nparts) * p.rms_inv_dim;   // E[x^2]
-      if (ln) {
-        r.mu[h] = sum_parts(p.ln_sum_in + (int64_t)row * p.rms_nparts, p.rms_nparts) * p.rms_inv_dim;
-        q = fmaxf(q - r.mu[h] * r.mu[h], 0.f);                                                          // variance
-      }
-      r.rs[h] *= rsqrtf(q + p.rms_eps);
-    }
+    r.rs[h] = row_factor<false>(p, row, r.mu[h]);
     int gr = row;
     if (p.conv_C > 0) {   // padded (to, ho16, wo16) row -> real output row, or nothing for the padding positions
       const int wo = gr % kConvLine, ho = (gr / kConvLine) % kConvLine, to = gr / (kConvLine * kConvLine);
@@ -363,43 +398,56 @@ enum : int {
   kEpiSwiglu,        // SwiGLU (gate-up)
 };
 
-// The global-memory operands of one 32-column slot of a variant: residuals, bias and RoPE table entries (zero where a
-// column or row is outside the output, or where the launch has no such operand).  They are loaded one slot ahead, so
-// their round trip overlaps the previous slot's math.  A residual that aliases the output is read at this thread's own
-// output positions only, before the thread writes them.
-struct SlotLoads {
-  uint32_t res[4][2];
-  float2 bias[4];
-  uint32_t rope[4][2];
+// Does 32-column slot c0 of a variant's tile have an operand slot (residual or RoPE table entries) in the operand ring?
+// The epilogue-operand warp and the consumers walk the same sequence.
+__device__ __forceinline__ bool slot_has_operand(const GemmParams& p, int c0) {
+  return p.epi == kEpiBiasRes || p.epi == kEpiResSumsq || (p.epi == kEpiRope && c0 < p.rope_cols);
+}
+template <int BN>
+__device__ __forceinline__ int epi_slots(const GemmParams& p, int n0) { return min(BN / 32, (p.N - n0 + 31) / 32); }
+
+// Byte offset of 4-byte word `word` of 16-byte chunk `chunk` in row r of a shared-memory tile of 64-byte rows that TMA
+// reads or writes with SWIZZLE_64B (the chunk index XOR bits 1-2 of the row), and the same for 32-byte rows with
+// SWIZZLE_32B (XOR bit 2 of the row).  The eight rows of a warp's fragment access then fall on distinct banks.
+__device__ __forceinline__ uint32_t swz64(int r, int chunk, int word) { return r * 64 + ((chunk ^ ((r >> 1) & 3)) << 4) + 4 * word; }
+__device__ __forceinline__ uint32_t swz32(int r, int chunk, int byte) { return r * 32 + ((chunk ^ ((r >> 2) & 1)) << 4) + byte; }
+
+// The epilogue variants' shared memory (see kEpiSmemBytes) and, right behind it, their barriers.  One base pointer: the
+// roles that use it run with few registers.
+static constexpr int kEpiBarriers = 4 + 2 * kOpSlots;
+struct EpiSmem {
+  uint8_t* base;
+  __device__ uint8_t* out(int cw, int i) const { return base + (2 * cw + i) * kStageTileBytes; }   // warp cw's tile i
+  __device__ uint8_t* op(int k) const { return base + kEpiOutBytes + k * kOpSlotBytes; }
+  __device__ float* rs(int b) const { return reinterpret_cast<float*>(base + kEpiOutBytes + kOpSlots * kOpSlotBytes) + b * 128; }
+  __device__ uint64_t* bar(int i) const { return reinterpret_cast<uint64_t*>(base + kEpiSmemBytes) + i; }
+  __device__ uint64_t* rs_full(int b) const { return bar(b); }                   // row-factor warps -> consumers
+  __device__ uint64_t* rs_empty(int b) const { return bar(2 + b); }              // consumer warps -> row-factor warps
+  __device__ uint64_t* op_full(int k) const { return bar(4 + k); }               // TMA -> consumers
+  __device__ uint64_t* op_empty(int k) const { return bar(4 + kOpSlots + k); }   // consumer warps -> operand warp
 };
-__device__ __forceinline__ void load_slot(SlotLoads& d, const GemmParams& p, const EpiRows& r, int n0, int s) {
+
+// bias of one 32-column slot (zero past N or without bias), loaded one slot ahead of its use
+__device__ __forceinline__ void load_bias(float2 (&b)[4], const GemmParams& p, int n0, int s) {
   const int t = threadIdx.x & 3;
-  const __nv_bfloat16* res = reinterpret_cast<const __nv_bfloat16*>(p.residual);
 #pragma unroll
   for (int jj = 0; jj < 4; ++jj) {
     const int c = n0 + 8 * (4 * s + jj) + 2 * t;
-    const bool col_ok = n0 + 8 * (4 * s + jj) < p.N;
-    d.bias[jj] = make_float2(0.f, 0.f);
-    if (p.bias != nullptr && col_ok) d.bias[jj] = __ldg(reinterpret_cast<const float2*>(p.bias + c));
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      d.res[jj][h] = 0u;
-      d.rope[jj][h] = 0u;
-      if (res != nullptr && col_ok && r.ok[h]) d.res[jj][h] = *reinterpret_cast<const uint32_t*>(res + (int64_t)r.rows[h] * p.ldr + c);
-      if (p.rope_tab != nullptr && col_ok && r.ok[h] && c < p.rope_cols)
-        d.rope[jj][h] = __ldg(p.rope_tab + (int64_t)(p.rope_pos0 + r.rows[h]) * (p.rope_D >> 1) + ((c % p.rope_D) >> 1));
-    }
+    b[jj] = make_float2(0.f, 0.f);
+    if (p.bias != nullptr && n0 + 8 * (4 * s + jj) < p.N) b[jj] = __ldg(reinterpret_cast<const float2*>(p.bias + c));
   }
 }
 
-// One 32-column slot s of a variant, from the slot's 16 accumulators v[] and its operands (loaded by the caller).
+// One 32-column slot s of a variant, from the slot's 16 accumulators v[], its operand words op[] (residual or RoPE table
+// entries, read from the operand ring) and bias, into the warp's staging tile at shared address `stage`.  Every value is
+// written; the TMA store clips rows and columns outside the output.
 template <int V>
-__device__ __forceinline__ void epilogue_slot(const float* v, const SlotLoads& ld, const GemmParams& p, const EpiRows& r,
-                                              int n0, int s, float k_log2e) {
+__device__ __forceinline__ void epilogue_slot(const float* v, const uint32_t (&op)[4][2], const float2 (&bias)[4],
+                                              const GemmParams& p, const EpiRows& r, int n0, int s, float k_log2e,
+                                              uint32_t stage) {
   constexpr bool kRes = V == kEpiBiasRes || V == kEpiResSumsq;
   constexpr bool kSumsq = V == kEpiResSumsq;
-  const int t = threadIdx.x & 3;
-  __nv_bfloat16* cb = reinterpret_cast<__nv_bfloat16*>(p.C);
+  const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
   float ssq[2] = {0.f, 0.f};
 #pragma unroll
   for (int jj = 0; jj < 4; ++jj) {
@@ -409,31 +457,32 @@ __device__ __forceinline__ void epilogue_slot(const float* v, const SlotLoads& l
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       float x0 = v[4 * jj + 2 * h], x1 = v[4 * jj + 2 * h + 1];
-      x0 = x0 * r.rs[h] + ld.bias[jj].x;   // a launch without bias adds 0, as the generic epilogue does
-      x1 = x1 * r.rs[h] + ld.bias[jj].y;
+      x0 = x0 * r.rs[h] + bias[jj].x;   // a launch without bias adds 0, as the generic epilogue does
+      x1 = x1 * r.rs[h] + bias[jj].y;
       const bool st_ok = col_ok && r.ok[h];
       if (V == kEpiSwiglu) {
+        // output columns 4 jj + t, 4 jj + t + 1 of the slot's 16: the even lane of a lane pair writes both lanes' outputs
         const float o = fast_sigmoid_mul(x0, 1.4426950408889634f) * x1;
         const float o_next = __shfl_down_sync(0xffffffffu, o, 1);
-        if (st_ok && (t & 1) == 0) *reinterpret_cast<uint32_t*>(cb + (int64_t)r.rows[h] * p.ldc + (c >> 1)) = pack_bf16(o, o_next);
+        if ((t & 1) == 0) sts32(stage + swz32(g + 8 * h, jj >> 1, 8 * (jj & 1) + 2 * t), pack_bf16(o, o_next));
         continue;
       }
       if (V == kEpiBiasSigmoid) { x0 = fast_sigmoid_mul(x0, k_log2e); x1 = fast_sigmoid_mul(x1, k_log2e); }
       if (V == kEpiBiasGeluErf) { x0 = act_apply(x0, VL2_ACT_GELU_ERF); x1 = act_apply(x1, VL2_ACT_GELU_ERF); }
       if (V == kEpiBiasGeluTanh) { x0 = gelu_tanh(x0); x1 = gelu_tanh(x1); }
       if (V == kEpiRope && c < p.rope_cols && st_ok) {
-        const uint32_t e = ld.rope[jj][h];
+        const uint32_t e = op[jj][h];
         const float co = bf16_lo(e), sn = bf16_hi(e);
         const float a = x0, b = x1;
         x0 = a * co - b * sn;
         x1 = b * co + a * sn;
       }
       if (kRes && st_ok) {
-        x0 += bf16_lo(ld.res[jj][h]);
-        x1 += bf16_hi(ld.res[jj][h]);
+        x0 += bf16_lo(op[jj][h]);
+        x1 += bf16_hi(op[jj][h]);
       }
       const uint32_t pk = pack_bf16(x0, x1);
-      if (st_ok) *reinterpret_cast<uint32_t*>(cb + (int64_t)r.rows[h] * p.ldc + c) = pk;
+      sts32(stage + swz64(g + 8 * h, jj, t), pk);
       if (kSumsq) {
         const float a0 = bf16_lo(pk), a1 = bf16_hi(pk);
         ssq[h] += a0 * a0 + a1 * a1;
@@ -451,40 +500,87 @@ __device__ __forceinline__ void epilogue_slot(const float* v, const SlotLoads& l
   }
 }
 
-// The epilogue of a consumer thread.  The variants loop over 32-column slots without unrolling: unrolled over a 128 x 256
-// tile, the nine of them made a ~20 k-instruction kernel.  Each iteration works on acc[0..15], indices fixed at compile
-// time, and then moves the array down by one slot (register moves; no run-time select of the slot's accumulators).  The
-// next slot's operands load while the current slot is computed.
+// The epilogue of a consumer thread.  `it` counts the CTA's items (row-factor buffer), `op_idx` the operand slots so far.
+//
+// A variant takes its row factors from shared memory and loops over 32-column slots without unrolling: unrolled over a
+// 128 x 256 tile, the nine of them made a ~20 k-instruction kernel.  Each iteration works on acc[0..15], indices fixed at
+// compile time, and then moves the array down by one slot (register moves; no run-time select of the slot's
+// accumulators).  Per slot a warp reads its operand words from the ring, writes its 16 x 32 piece into one of its two
+// staging tiles and one lane stores that by TMA without waiting for it; a staging tile is rewritten once the store that
+// read it two slots ago has finished reading (the previous tile's stores, a k-loop ago, before the first slot).  A residual that aliases the output is in shared memory before the tile's
+// stores of the same positions are issued.
 template <int BN>
-__device__ __forceinline__ void run_epilogue(float (&acc)[BN / 2], const GemmParams& p, int m0, int n0, int rloc,
+__device__ __forceinline__ void run_epilogue(float (&acc)[BN / 2], const GemmParams& p, const CUtensorMap* tmap_c,
+                                             const EpiSmem& sm, int m0, int n0, int rloc, int it, uint32_t& op_idx,
                                              long long* tr) {
-  const EpiRows r = epi_rows(p, m0, rloc);
   if (p.epi == kEpiGeneric) {
-    gemm_epilogue<BN>(acc, p, r, n0, tr);
+    gemm_epilogue<BN>(acc, p, epi_rows(p, m0, rloc), n0, tr);
     return;
   }
   if (tr != nullptr) { tr[1] = -1; tr[2] = -1; }   // generic-only trace points: not recorded by this launch
+  const int lane = threadIdx.x & 31, t = lane & 3;
+  const int cw = (threadIdx.x - 128) >> 5;         // consumer warp 0..7: rows [16 cw, 16 cw + 16) of the tile
+  EpiRows r;
+  {
+    const int b = it & 1;
+    mbar_wait(sm.rs_full(b), (it >> 1) & 1);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      r.rows[h] = m0 + rloc + 8 * h;
+      r.ok[h] = r.rows[h] < p.M;
+      r.rs[h] = sm.rs(b)[rloc + 8 * h];
+      r.mu[h] = 0.f;
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(sm.rs_empty(b));
+  }
   const float k_log2e = p.act == VL2_ACT_QUICK_GELU ? 1.702f * 1.4426950408889634f : 1.4426950408889634f;
-  const int nslots = min(BN / 32, (p.N - n0 + 31) / 32);
-  SlotLoads cur, next = {};
-  load_slot(cur, p, r, n0, 0);
+  const int nslots = epi_slots<BN>(p, n0);
+  const bool swiglu = p.epi == kEpiSwiglu;
+  float2 bias[4], bias_next[4];
+  load_bias(bias, p, n0, 0);
+  if (lane == 0) bulk_wait_read<0>();
 #pragma unroll 1
   for (int s = 0; s < nslots; ++s) {
-    if (s + 1 < nslots) load_slot(next, p, r, n0, s + 1);
+    if (s + 1 < nslots) load_bias(bias_next, p, n0, s + 1);
+    uint32_t op[4][2] = {};
+    if (slot_has_operand(p, n0 + 32 * s)) {
+      const int k = op_idx % kOpSlots;
+      mbar_wait(sm.op_full(k), (op_idx / kOpSlots) & 1);
+      const uint32_t base = smem_u32(sm.op(k));
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) op[jj][h] = lds32(base + swz64(rloc + 8 * h, jj, t));
+      __syncwarp();
+      if (lane == 0) mbar_arrive(sm.op_empty(k));
+      ++op_idx;
+    }
+    uint8_t* stage = sm.out(cw, s & 1);
+    if (lane == 0 && s >= 2) bulk_wait_read<1>();   // the store that read this staging tile (slot s - 2) is done reading it
+    __syncwarp();
+    const uint32_t st = smem_u32(stage);
     switch (p.epi) {   // uniform over the launch
-      case kEpiNone: epilogue_slot<kEpiNone>(acc, cur, p, r, n0, s, k_log2e); break;
-      case kEpiBias: epilogue_slot<kEpiBias>(acc, cur, p, r, n0, s, k_log2e); break;
-      case kEpiBiasSigmoid: epilogue_slot<kEpiBiasSigmoid>(acc, cur, p, r, n0, s, k_log2e); break;
-      case kEpiBiasGeluErf: epilogue_slot<kEpiBiasGeluErf>(acc, cur, p, r, n0, s, k_log2e); break;
-      case kEpiBiasGeluTanh: epilogue_slot<kEpiBiasGeluTanh>(acc, cur, p, r, n0, s, k_log2e); break;
-      case kEpiBiasRes: epilogue_slot<kEpiBiasRes>(acc, cur, p, r, n0, s, k_log2e); break;
-      case kEpiResSumsq: epilogue_slot<kEpiResSumsq>(acc, cur, p, r, n0, s, k_log2e); break;
-      case kEpiRope: epilogue_slot<kEpiRope>(acc, cur, p, r, n0, s, k_log2e); break;
-      default: epilogue_slot<kEpiSwiglu>(acc, cur, p, r, n0, s, k_log2e); break;
+      case kEpiNone: epilogue_slot<kEpiNone>(acc, op, bias, p, r, n0, s, k_log2e, st); break;
+      case kEpiBias: epilogue_slot<kEpiBias>(acc, op, bias, p, r, n0, s, k_log2e, st); break;
+      case kEpiBiasSigmoid: epilogue_slot<kEpiBiasSigmoid>(acc, op, bias, p, r, n0, s, k_log2e, st); break;
+      case kEpiBiasGeluErf: epilogue_slot<kEpiBiasGeluErf>(acc, op, bias, p, r, n0, s, k_log2e, st); break;
+      case kEpiBiasGeluTanh: epilogue_slot<kEpiBiasGeluTanh>(acc, op, bias, p, r, n0, s, k_log2e, st); break;
+      case kEpiBiasRes: epilogue_slot<kEpiBiasRes>(acc, op, bias, p, r, n0, s, k_log2e, st); break;
+      case kEpiResSumsq: epilogue_slot<kEpiResSumsq>(acc, op, bias, p, r, n0, s, k_log2e, st); break;
+      case kEpiRope: epilogue_slot<kEpiRope>(acc, op, bias, p, r, n0, s, k_log2e, st); break;
+      default: epilogue_slot<kEpiSwiglu>(acc, op, bias, p, r, n0, s, k_log2e, st); break;
+    }
+    fence_proxy_async_smem();   // the warp's writes -> visible to the TMA store
+    __syncwarp();
+    if (lane == 0) {
+      tma_store_2d(tmap_c, stage, swiglu ? (n0 >> 1) + 16 * s : n0 + 32 * s, m0 + 16 * cw);
+      bulk_commit_group();
     }
 #pragma unroll
     for (int i = 0; i + 16 < BN / 2; ++i) acc[i] = acc[i + 16];
-    cur = next;
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj) bias[jj] = bias_next[jj];
     if (s == 0) trace_point(tr, 3);
   }
 }
@@ -492,6 +588,7 @@ __device__ __forceinline__ void run_epilogue(float (&acc)[BN / 2], const GemmPar
 template <int BN, bool PAIR>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                       const __grid_constant__ CUtensorMap tmap_c, const __grid_constant__ CUtensorMap tmap_op,
                        const GemmParams p) {
   using Cfg = GemmCfg<BN, PAIR>;
   const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
@@ -504,7 +601,8 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
   if ((smem_u32(smem) & 1023u) != 0) { asm volatile("trap;"); }
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + Cfg::kStages * Cfg::kStageBytesA;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
+  const EpiSmem es{smem + Cfg::kStages * Cfg::kStageBytes};   // 1024-byte aligned: stage sizes are multiples of 1 KB
+  uint64_t* bars = es.bar(kEpiBarriers);
   uint64_t* full_bar = bars;                        // [kStages]  TMA -> consumers
   uint64_t* empty_bar = bars + Cfg::kStages;        // [kStages]  consumers (of both CTAs of a pair) -> TMA
 
@@ -519,6 +617,18 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     for (int i = 0; i < Cfg::kStages; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], Cfg::kEmptyArrivals);
+    }
+    for (int i = 0; i < 2; ++i) {
+      mbar_init(es.rs_full(i), 64);
+      mbar_init(es.rs_empty(i), kConsumerThreads / 32);
+    }
+    for (int i = 0; i < kOpSlots; ++i) {
+      mbar_init(es.op_full(i), 1);
+      mbar_init(es.op_empty(i), kConsumerThreads / 32);
+    }
+    if (p.epi != kEpiGeneric) {
+      tma_prefetch_desc(&tmap_c);
+      if (p.residual != nullptr || p.rope_tab != nullptr) tma_prefetch_desc(&tmap_op);
     }
     fence_barrier_init();
   }
@@ -561,6 +671,44 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
           if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
         }
       }
+    } else if (warp == 1 && lane == 0 && p.epi != kEpiGeneric && (p.residual != nullptr || p.rope_tab != nullptr)) {
+      // ===================== epilogue operands of a variant: residual / RoPE-table slots =====================
+      // The tile's operand slots into the ring by TMA, the first ones while the tile's k-loop runs.  Independent of the
+      // A/B producer, so the A/B ring never waits on epilogue buffers.
+      uint32_t op_idx = 0;
+      for (int item = tile0; item < p.num_items; item += tile_stride) {
+        const WorkItem w = decode_item(item, p, num_k_blocks);   // a variant's launch is not split: item = tile
+        const int m0 = (w.tile % p.num_m_tiles) * kTileM + (int)rank * BM;
+        const int n0 = (w.tile / p.num_m_tiles) * BN;
+        const int nslots = epi_slots<BN>(p, n0);
+        for (int s = 0; s < nslots; ++s) {
+          const int c0 = n0 + 32 * s;
+          if (!slot_has_operand(p, c0)) continue;
+          const int k = op_idx % kOpSlots;
+          mbar_wait_parked(es.op_empty(k), ((op_idx / kOpSlots) & 1) ^ 1);
+          mbar_arrive_expect_tx(es.op_full(k), kOpSlotBytes);
+          // the RoPE table [pos][D / 2] of (cos, sin) pairs is mapped as 16-bit pairs: entry e = columns 2 e, 2 e + 1
+          if (p.epi == kEpiRope) tma_load_2d(es.op(k), &tmap_op, es.op_full(k), c0 % p.rope_D, p.rope_pos0 + m0);
+          else tma_load_2d(es.op(k), &tmap_op, es.op_full(k), c0, m0);
+          ++op_idx;
+        }
+      }
+    } else if (warp >= 2 && p.epi != kEpiGeneric) {
+      // ===================== epilogue operands of a variant: row factors =====================
+      // The tile's 128 row factors (rows i and i + 64 of thread i), with the generic epilogue's arithmetic, into the
+      // tile's half of the row-factor buffer while its k-loop runs: the consumers' epilogue starts without a row prologue.
+      int it = 0;
+      for (int tile = tile0; tile < p.num_items; tile += tile_stride, ++it) {   // a variant's launch is not split
+        const int m0 = (tile % p.num_m_tiles) * kTileM + (int)rank * BM;
+        const int b = it & 1;
+        mbar_wait_parked(es.rs_empty(b), ((it >> 1) & 1) ^ 1);
+#pragma unroll 1
+        for (int r = threadIdx.x - 64; r < BM; r += 64) {
+          float mu;
+          es.rs(b)[r] = row_factor<true>(p, m0 + r, mu);
+        }
+        mbar_arrive(es.rs_full(b));
+      }
     }
   } else {
     setmaxnreg_inc<232>();
@@ -574,6 +722,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     int stage = 0;
     uint32_t phase = 0;
     int it = 0;
+    uint32_t op_idx = 0;
     float acc[Cfg::kAcc];
     for (int item = tile0; item < p.num_items; item += tile_stride, ++it) {
       const WorkItem w = decode_item(item, p, num_k_blocks);
@@ -636,8 +785,15 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
         consumer_sync();   // every thread has consumed the partials: re-arm the counter for the next launch
         if (ctid == 0) *flag = 0u;
       }
-      run_epilogue<BN>(acc, p, m0, n0, rloc, (tr && it < 7) ? g_gemm_trace + 8 * it : nullptr);
-      if (tr && it < 7) { g_gemm_trace[8 * it + 6] = clock64(); g_gemm_trace[0] = it + 1; }
+      run_epilogue<BN>(acc, p, &tmap_c, es, m0, n0, rloc, it, op_idx, (tr && it < 7) ? g_gemm_trace + 8 * it : nullptr);
+      // the warp's TMA stores are complete before the CTA's shared memory goes away (inside the loop: placed after it, the
+      // wait made ptxas hold the consumers to the launch's 168 registers)
+      if (item + tile_stride >= p.num_items && lane == 0) bulk_wait_all();
+      if (tr && it < 7) {
+        bulk_wait_read_all();   // the variants' stores: issued by this thread, done reading shared memory
+        g_gemm_trace[8 * it + 6] = clock64();
+        g_gemm_trace[0] = it + 1;
+      }
     }
   }
   if (PAIR) cluster_sync_all();   // no CTA leaves while its peer may still multicast into it or arrive on its barriers
@@ -657,7 +813,7 @@ static constexpr double kIngestBytesPerClk = 64.0;
 
 static double kb_cycles(int bn, bool pair) {
   const double stage_bytes = 16384.0 + bn * 128.0;
-  int stages = (int)((227 * 1024 - 1024) / stage_bytes);
+  int stages = (int)((kSmemLimit - 1024 - kEpiSmemBytes) / stage_bytes);   // GemmCfg::kStages
   if (stages > 8) stages = 8;
   const double mma = 128.0 * bn * 64.0 / 1024.0 + 200.0;
   const double ingest = (16384.0 + (pair ? bn / 2 : bn) * 128.0) / kIngestBytesPerClk;
@@ -813,10 +969,37 @@ static int launch_gemm(const vl2_gemm_args* a, cudaStream_t stream) {
   }
   p.num_items = p.split_first + (tiles - p.split_first) * p.split_s;
   p.epi = (p.split_s > 1 || a->reserved2 == 778 || a->reserved2 == 779) ? kEpiGeneric : classify_epilogue(a);
+  // A variant's output leaves by TMA stores of 16-row slots whose map clips the M and N tails (and keeps a strided view's
+  // columns past N untouched); its residual or RoPE table arrives by TMA loads of 128-row slots.  vl2_gemm_bf16 requires
+  // 16-byte aligned pointers and leading dimensions that are multiples of 8 elements, so every such launch has the maps.
+  CUtensorMap tc, top;
+  memset(&tc, 0, sizeof(tc));
+  memset(&top, 0, sizeof(top));
+  if (p.epi != kEpiGeneric) {
+    const bool swiglu = p.epi == kEpiSwiglu;
+    uint64_t dims[2] = {(uint64_t)(swiglu ? a->N / 2 : a->N), (uint64_t)a->M};
+    uint64_t str[1] = {(uint64_t)a->ldc * 2};
+    uint32_t box[2] = {swiglu ? 16u : 32u, 16u};
+    int rc = make_tmap_bf16(&tc, a->C, 2, dims, str, box, swiglu ? 32 : 64);
+    if (rc) return rc;
+    if (p.epi == kEpiRope) {
+      uint64_t rdims[2] = {(uint64_t)a->rope_D, (uint64_t)a->rope_pos0 + (uint64_t)a->M};   // the positions it reads
+      uint64_t rstr[1] = {(uint64_t)a->rope_D * 2};
+      uint32_t rbox[2] = {32u, (uint32_t)BM};
+      rc = make_tmap_bf16(&top, a->rope_tab, 2, rdims, rstr, rbox, 64);
+    } else if (a->residual != nullptr) {
+      uint64_t rdims[2] = {(uint64_t)a->N, (uint64_t)a->M};
+      uint64_t rstr[1] = {(uint64_t)a->ldr * 2};
+      uint32_t rbox[2] = {32u, (uint32_t)BM};
+      rc = make_tmap_bf16(&top, a->residual, 2, rdims, rstr, rbox, 64);
+    }
+    if (rc) return rc;
+  }
   const int units = p.num_items < slots ? p.num_items : slots;
   const dim3 grid(PAIR ? 2 * units : units), block(kGemmThreads);
   VL2_SMEM_OPT_IN((gemm_bf16_wgmma_kernel<BN, PAIR>), Cfg::kSmemBytes);
-  VL2_CHECK_CUDA(launch_kernel(gemm_bf16_wgmma_kernel<BN, PAIR>, grid, block, Cfg::kSmemBytes, stream, PAIR ? 2 : 1, ta, tb, p));
+  VL2_CHECK_CUDA(launch_kernel(gemm_bf16_wgmma_kernel<BN, PAIR>, grid, block, Cfg::kSmemBytes, stream, PAIR ? 2 : 1, ta, tb, tc, top,
+                                 p));
   VL2_CHECK_LAUNCH("gemm_bf16_wgmma_kernel");
   return VL2_OK;
 }

@@ -89,8 +89,11 @@ int make_tmap_bf16(CUtensorMap* map, const void* base, int rank, const uint64_t*
 #else
   const CUtensorMapDataType elem_type = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
 #endif
+  const CUtensorMapSwizzle swz = swizzle_bytes == 32   ? CU_TENSOR_MAP_SWIZZLE_32B
+                                 : swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
+                                                       : CU_TENSOR_MAP_SWIZZLE_128B;
   CUresult r = enc(map, elem_type, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bx, es,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, swz,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS)

@@ -16,8 +16,8 @@ int sm_count();        // of the CURRENT device (cached per device)
 int device_slot();     // cudaGetDevice(), clamped to [0, kMaxDevices): index of per-device host caches
 static constexpr int kMaxDevices = 64;
 
-// Encode a tiled bf16 tensor map with 128-byte swizzle (swizzle_bytes = 64: 64-byte swizzle, for boxes whose rows are
-// 64 bytes) and zero OOB fill.  dims/strides are innermost-first; strides (bytes) are given for dims 1..rank-1.
+// Encode a tiled bf16 tensor map with 128-byte swizzle (swizzle_bytes = 64 / 32: 64- / 32-byte swizzle, for boxes whose
+// rows are 64 / 32 bytes) and zero OOB fill.  dims/strides are innermost-first; strides (bytes) are given for dims 1..rank-1.
 int make_tmap_bf16(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                    const uint32_t* box, int swizzle_bytes = 128);
 
