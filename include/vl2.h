@@ -410,6 +410,8 @@ int vl2_patch_embed(const vl2_patch_embed_args* args, void* stream);
  * kernel broadcasts with peer stores instead of multimem.st).  Rank r reduces rows
  * [r*ceil(S/world), ...) and writes them to every rank.  pads: >= 17 zero-initialised uint32 per rank; `epoch` = 1, 2, 3, ...
  * counts the calls that used these pads (the same on every rank).  Not CUDA-graph replayable (epoch is a launch argument).
+ * VL2_E_BADSHAPE: world outside [1, 8], rank outside [0, world), S or H not positive, H % 8 != 0, epoch 0, part_mc without
+ * xout_mc and stats_mc, or a missing buffer of a rank < world; VL2_E_BADALIGN: part[r] or xout[r] not 16-byte aligned.
  * ---------------------------------------------------------------------------------------------------------- */
 typedef struct vl2_tp_allreduce_args {
   const void* part[8];

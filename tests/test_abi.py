@@ -75,6 +75,45 @@ def test_argument_validation_without_gpu(lib):
         assert getattr(lib, name)(*args) == code, (name, args, lib.vl2_last_error())
 
 
+def _tp_args(**kw):
+    """vl2_tp_allreduce_args of rank 0 of 2 over fake, 16-byte aligned buffers; `kw` overrides fields."""
+    from videollama2_b200._lib import TpAllReduceArgs
+    a = TpAllReduceArgs(rank=0, world=2, S=4, H=64, epoch=1, inswitch_reduce=0)
+    for r in range(8):
+        a.part[r], a.xout[r], a.stats[r], a.pads[r] = A16, A16 + 4096, A16 + 8192, A16 + 12288
+    for k, v in kw.items():
+        if isinstance(v, tuple):                  # (array field, index, value)
+            getattr(a, k)[v[0]] = v[1]
+        else:
+            setattr(a, k, v)
+    return a
+
+
+TP_ARGUMENT_CASES = [
+    (dict(world=0), BADSHAPE), (dict(world=9), BADSHAPE),
+    (dict(rank=2), BADSHAPE), (dict(rank=-1), BADSHAPE),
+    (dict(S=0), BADSHAPE), (dict(H=60), BADSHAPE), (dict(H=0), BADSHAPE),
+    (dict(epoch=0), BADSHAPE),
+    (dict(part_mc=A16), BADSHAPE),                              # multicast part without multicast xout / stats
+    (dict(part_mc=A16, xout_mc=A16), BADSHAPE),
+    (dict(part=(1, None)), BADSHAPE), (dict(xout=(1, None)), BADSHAPE), (dict(stats=(1, None)), BADSHAPE),
+    (dict(pads=(1, None)), BADSHAPE),
+    (dict(part=(1, MIS)), BADALIGN), (dict(xout=(0, MIS)), BADALIGN),
+]
+
+
+def test_tp_allreduce_argument_validation_without_gpu(lib):
+    """vl2_tp_allreduce_stats refuses, before any CUDA call: a world outside 1..8, a rank outside the world, S or H not
+    positive, H % 8 != 0, epoch 0 (the pads start at 0: nothing would wait), a multicast part address without the other
+    two, a missing buffer of a rank in the world (VL2_E_BADSHAPE), and a part or xout buffer that is not 16-byte aligned
+    (VL2_E_BADALIGN), each with a message naming the call."""
+    for kw, code in TP_ARGUMENT_CASES:
+        a = _tp_args(**kw)
+        assert lib.vl2_tp_allreduce_stats(ctypes.byref(a), None) == code, (kw, lib.vl2_last_error())
+        assert lib.vl2_last_error().startswith(b"vl2_tp_allreduce_stats: "), kw
+    assert lib.vl2_tp_allreduce_stats(None, None) == BADSHAPE
+
+
 def test_ops_refuse_cpu_tensors():
     import torch
     from videollama2_b200 import ops

@@ -1,8 +1,9 @@
 """Self-tests of the checks in test_kernels_exact_gpu.py and test_rowops_decode_exact_gpu.py, on the CPU: plant the
 faults a whole-tensor relL2 < 6e-3 lets through into a correct fp64 result and show that the element-wise checker
 rejects each of them, while it accepts the correctly rounded result.  Also checks on the CPU that the attention routing
-problems route (fp64 softmax is one-hot on the target) and that the RoPE table matcher tells rounding noise from a
-wrong table."""
+problems route (fp64 softmax is one-hot on the target), that the RoPE table matcher tells rounding noise from a
+wrong table, and that the all-reduce expectation of test_tp_allreduce_gpu.py pins the rank order, the fp32 accumulation
+and the statistics of the rounded sum."""
 import math
 
 import pytest
@@ -13,6 +14,7 @@ from test_kernels_exact_gpu import (FP16_MAX, STORAGE_TYPES, _ln_rows_bound, _ro
                                     storage_params, to_storage_exact)
 from test_rowops_decode_exact_gpu import (ROPE_POSITIONS, ROPE_THETA, rope_angles_fp32, rope_table_mismatches,
                                           rope_table_parts)
+from test_tp_allreduce_gpu import expected_sum, make_partials, stats_violations, to_storage
 
 CPU = torch.device("cpu")
 
@@ -217,3 +219,31 @@ def test_fp16_overflow_reference():
     want = torch.tensor([FP16_MAX, FP16_MAX, math.inf, -math.inf, math.inf, -FP16_MAX, -FP16_MAX,
                          2.0 ** -24, 2.0 * 2.0 ** -24, 0.0], dtype=torch.float64)
     assert torch.equal(got, want)
+
+
+@pytest.mark.parametrize("dt", STORAGE_TYPES, ids=["bf16", "fp16"])
+def test_allreduce_expectation_rejects_other_orders_and_roundings(dt):
+    """On the probe rows of make_partials (every fourth row, columns 0 and 1), the expected all-reduce changes when the
+    ranks are summed in reverse order or exactly (fp64) before the one rounding; anywhere, when every step is rounded
+    to the storage type.  Statistics taken from the fp32 sum before its rounding are rejected, those of the rounded
+    sum accepted."""
+    import numpy as np
+    p = make_partials(3, 16, 64, dt, seed=7)
+    want = expected_sum(p, dt)
+
+    def differ(a, b):
+        return int((a.view(np.uint32) != b.view(np.uint32)).sum())
+    assert differ(expected_sum(p[::-1], dt)[0::4, :2], want[0::4, :2]) > 0
+    with np.errstate(invalid="ignore", over="ignore"):
+        exact = to_storage(p.astype(np.float64).sum(0).astype(np.float32), dt)
+        step = np.zeros(p.shape[1:], np.float32)
+        acc = np.zeros(p.shape[1:], np.float32)
+        for q in p:
+            step = to_storage(step + q, dt)
+            acc += q
+        unrounded_stats = (acc.astype(np.float64) ** 2).sum(1).astype(np.float32)
+    assert differ(exact[0::4, :2], want[0::4, :2]) > 0
+    assert differ(step, want) > 0
+    good = (want.astype(np.float64) ** 2).sum(1).astype(np.float32)
+    assert stats_violations(good, want).size == 0
+    assert stats_violations(unrounded_stats, want).size > 0
