@@ -251,6 +251,33 @@ int vl2_sample_token(const float* logits, int V, const vl2_sample_params* params
                      int64_t counter_add, int64_t* token_out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Per-step scores for generate(output_scores / output_logits): fp32 rows [V] recorded into per-call buffers
+ * [capacity, V], row `slot` at offset slot * V.  The destination is described by a parameter block in device memory, so
+ * one captured graph serves buffers of any size: a slot outside [0, capacity) writes nothing, nor does a null buffer or
+ * a block whose V differs from the launch's.
+ * ---------------------------------------------------------------------------------------------------------- */
+typedef struct vl2_score_record_params {
+  float* scores;        /* device [capacity, V]: the processed (greedy) or warped (sampled) rows, or null */
+  float* logits;        /* device [capacity, V]: the raw lm_head rows, or null */
+  int64_t capacity;     /* rows in each buffer */
+  int32_t V;
+  int32_t reserved;
+} vl2_score_record_params;
+enum { VL2_RECORD_LOGITS = 0, VL2_RECORD_SCORES = 1 };
+/* Copy row[0 .. V) into the `which` buffer (VL2_RECORD_LOGITS / VL2_RECORD_SCORES) of `params` at slot
+ * *step_dev + add.  V outside [1, 262144] or another `which`: VL2_E_BADSHAPE; row 4-byte aligned, params and step_dev
+ * 8-byte aligned and not null (VL2_E_BADALIGN). */
+int vl2_record_row(const float* row, int V, const vl2_score_record_params* params, int which, const int64_t* step_dev,
+                   int64_t add, void* stream);
+/* vl2_sample_token that also writes the warped row HF's sampler returns as `scores` into record->scores at slot
+ * n = *counter_dev + counter_add: the bits of l / T (IEEE fp32 division; -0.0 stays -0.0) where the token is kept by
+ * top-k and top-p, -inf elsewhere.  The token is vl2_sample_token's for the same arguments.  Argument errors as
+ * vl2_sample_token's; record null or not 8-byte aligned: VL2_E_BADALIGN. */
+int vl2_sample_token_scored(const float* logits, int V, const vl2_sample_params* params, const int64_t* counter_dev,
+                            int64_t counter_add, int64_t* token_out, const vl2_score_record_params* record,
+                            void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Logits processors for generate(): HF's RepetitionPenaltyLogitsProcessor, NoRepeatNGramLogitsProcessor,
  * NoBadWordsLogitsProcessor, MinNewTokensLengthLogitsProcessor and SuppressTokensLogitsProcessor (restated by
  * videollama2_b200/sampling.py:process_logits), in place on one fp32 logits row [V], V <= 262144, one launch,

@@ -18,7 +18,7 @@ SYMBOLS = [
     "vl2_patch_im2col", "vl2_clip_embed_finish",
     "vl2_dwconv3x3_ln_silu", "vl2_se_scale", "vl2_conv3d_im2col",
     "vl2_rope_inplace", "vl2_embed_splice", "vl2_tp_allreduce_stats", "vl2_patch_embed",
-    "vl2_sample_token", "vl2_process_logits",
+    "vl2_sample_token", "vl2_process_logits", "vl2_record_row", "vl2_sample_token_scored",
 ]
 
 ACT_NONE, ACT_QUICK_GELU, ACT_SILU, ACT_GELU_ERF, ACT_SWIGLU, ACT_GELU_TANH = 0, 1, 2, 3, 4, 5
@@ -80,6 +80,14 @@ class LogitsProcessParams(C.Structure):
     _fields_ = [("repetition_penalty", C.c_float), ("no_repeat_ngram_size", C.c_int32), ("min_new_tokens", C.c_int64),
                 ("n_eos", C.c_int32), ("n_suppress", C.c_int32), ("n_bad", C.c_int32), ("reserved", C.c_int32),
                 ("eos_ids", C.c_void_p), ("suppress_ids", C.c_void_p), ("bad_offsets", C.c_void_p), ("bad_ids", C.c_void_p)]
+
+
+class ScoreRecordParams(C.Structure):
+    _fields_ = [("scores", C.c_void_p), ("logits", C.c_void_p), ("capacity", C.c_int64), ("V", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
+RECORD_LOGITS, RECORD_SCORES = 0, 1     # vl2_record_row's `which`
 
 
 class Vl2Error(RuntimeError):
@@ -162,6 +170,8 @@ def load(dtype=None) -> C.CDLL:
         "vl2_patch_embed": [C.POINTER(PatchEmbedArgs), vp],
         "vl2_sample_token": [vp, i32, vp, vp, i64, vp, vp],
         "vl2_process_logits": [vp, i32, vp, vp, vp, i64, vp],
+        "vl2_record_row": [vp, i32, vp, i32, vp, i64, vp],
+        "vl2_sample_token_scored": [vp, i32, vp, vp, i64, vp, vp, vp],
     }
     for name, argtypes in sigs.items():
         fn = getattr(lib, name)

@@ -142,11 +142,13 @@ __device__ __forceinline__ void radix_pick(const unsigned long long* hist, int n
 }
 
 // SMEM: the row's keys stay in dynamic shared memory after pass 1 (V <= kSampleSmemV); otherwise every pass recomputes
-// them from the logits (an L2-resident re-read).
-template <bool SMEM>
+// them from the logits (an L2-resident re-read).  SCORED: once the thresholds are known, one more pass writes the warped
+// row (l / T where kept, -inf elsewhere) to slot n of rec->scores; without it `rec` is not read.
+template <bool SMEM, bool SCORED>
 __global__ void __launch_bounds__(kSampleThreads, 1)
 sample_token_kernel(const float* __restrict__ logits, int V, const vl2_sample_params* __restrict__ params,
-                    const int64_t* __restrict__ counter_dev, int64_t counter_add, int64_t* __restrict__ out) {
+                    const int64_t* __restrict__ counter_dev, int64_t counter_add, int64_t* __restrict__ out,
+                    const vl2_score_record_params* __restrict__ rec) {
   extern __shared__ uint32_t keys[];
   __shared__ unsigned long long hist[kSampleBins];
   __shared__ unsigned long long red[kSampleWarps];
@@ -259,6 +261,18 @@ sample_token_kernel(const float* __restrict__ logits, int V, const vl2_sample_pa
     thr = max(thr, prefix);
   }
 
+  if (SCORED) {
+    const int64_t slot = (int64_t)n;
+    float* dst = rec->scores;
+    if (dst != nullptr && rec->V == V && slot >= 0 && slot < rec->capacity) {
+      dst += slot * (int64_t)V;
+      for (int i = tid; i < V; i += kSampleThreads) {
+        const float s = __fdiv_rn(__ldg(logits + i), T);          // unclean: -0.0 and NaN stay as torch leaves them
+        dst[i] = (SMEM ? keys[i] : score_key(clean_score(s))) >= thr ? s : -INFINITY;
+      }
+    }
+  }
+
   // draw: warp w owns the index range [w * L, (w + 1) * L); the kept mass of each range, then one warp walks the range
   // that holds the target in index order
   auto weight_at = [&](int i) -> unsigned long long {
@@ -331,21 +345,37 @@ sample_token_kernel(const float* __restrict__ logits, int V, const vl2_sample_pa
 
 using namespace vl2;
 
-extern "C" int vl2_sample_token(const float* logits, int V, const vl2_sample_params* params, const int64_t* counter_dev,
-                                int64_t counter_add, int64_t* token_out, void* stream) {
-  VL2_REQUIRE(V > 0 && V <= kSampleMaxV, VL2_E_BADSHAPE, "vl2_sample_token: V = %d outside [1, %d]", V, kSampleMaxV);
-  VL2_REQUIRE(logits && params && counter_dev && token_out, VL2_E_BADALIGN, "vl2_sample_token: null pointer");
+template <bool SCORED>
+static int sample_token_launch(const char* fn, const float* logits, int V, const vl2_sample_params* params,
+                               const int64_t* counter_dev, int64_t counter_add, int64_t* token_out,
+                               const vl2_score_record_params* rec, void* stream) {
+  VL2_REQUIRE(V > 0 && V <= kSampleMaxV, VL2_E_BADSHAPE, "%s: V = %d outside [1, %d]", fn, V, kSampleMaxV);
+  VL2_REQUIRE(logits && params && counter_dev && token_out && (rec || !SCORED), VL2_E_BADALIGN, "%s: null pointer", fn);
   VL2_REQUIRE((reinterpret_cast<uintptr_t>(logits) & 3) == 0 && (reinterpret_cast<uintptr_t>(params) & 7) == 0 &&
-                  (reinterpret_cast<uintptr_t>(counter_dev) & 7) == 0 && (reinterpret_cast<uintptr_t>(token_out) & 7) == 0,
-              VL2_E_BADALIGN, "vl2_sample_token: logits need 4-byte, params / counter / token 8-byte alignment");
+                  (reinterpret_cast<uintptr_t>(counter_dev) & 7) == 0 && (reinterpret_cast<uintptr_t>(token_out) & 7) == 0 &&
+                  (reinterpret_cast<uintptr_t>(rec) & 7) == 0,
+              VL2_E_BADALIGN, "%s: logits need 4-byte, params / counter / token / record 8-byte alignment", fn);
   if (V <= kSampleSmemV) {
-    VL2_SMEM_OPT_IN(sample_token_kernel<true>, kSampleSmemV * 4);
-    launch_kernel(sample_token_kernel<true>, dim3(1), dim3(kSampleThreads), (size_t)V * 4, (cudaStream_t)stream, 1, logits,
-                  V, params, counter_dev, counter_add, token_out);
+    VL2_SMEM_OPT_IN((sample_token_kernel<true, SCORED>), kSampleSmemV * 4);
+    launch_kernel(sample_token_kernel<true, SCORED>, dim3(1), dim3(kSampleThreads), (size_t)V * 4, (cudaStream_t)stream,
+                  1, logits, V, params, counter_dev, counter_add, token_out, rec);
   } else {
-    launch_kernel(sample_token_kernel<false>, dim3(1), dim3(kSampleThreads), 0, (cudaStream_t)stream, 1, logits, V, params,
-                  counter_dev, counter_add, token_out);
+    launch_kernel(sample_token_kernel<false, SCORED>, dim3(1), dim3(kSampleThreads), 0, (cudaStream_t)stream, 1, logits,
+                  V, params, counter_dev, counter_add, token_out, rec);
   }
   VL2_CHECK_LAUNCH("sample_token_kernel");
   return VL2_OK;
+}
+
+extern "C" int vl2_sample_token(const float* logits, int V, const vl2_sample_params* params, const int64_t* counter_dev,
+                                int64_t counter_add, int64_t* token_out, void* stream) {
+  return sample_token_launch<false>("vl2_sample_token", logits, V, params, counter_dev, counter_add, token_out, nullptr,
+                                    stream);
+}
+
+extern "C" int vl2_sample_token_scored(const float* logits, int V, const vl2_sample_params* params,
+                                       const int64_t* counter_dev, int64_t counter_add, int64_t* token_out,
+                                       const vl2_score_record_params* record, void* stream) {
+  return sample_token_launch<true>("vl2_sample_token_scored", logits, V, params, counter_dev, counter_add, token_out,
+                                   record, stream);
 }

@@ -13,7 +13,7 @@ from typing import Dict, List, Optional
 
 import torch
 
-from .. import ops
+from .. import _lib, ops
 
 
 class DecoderEngine:
@@ -36,12 +36,16 @@ class DecoderEngine:
         self._decode_graph_sampled = None   # the same step ending in vl2_sample_token instead of the arg-max
         # the greedy and sampled steps with vl2_process_logits in front of the token choice (captured on first use only)
         self._decode_graph_processed = self._decode_graph_sampled_processed = None
+        # the four steps above, also recording their rows for generate(output_scores / output_logits), keyed by
+        # (sampled, processed) and captured on first use only
+        self._decode_graphs_recorded: Dict[tuple, tuple] = {}
         self._decode_bufs = None    # (tok_dev, pos_dev, stage, gen_buf, step_dev): device state the graphs share
         self._decode_log = None     # (device id buffer, device step counter) the graphs append their tokens to
         self._decode_hist = None    # new token 0 followed by the id log (gen_buf is its view from index 1)
         self._sample_params = None  # device vl2_sample_params the sampled graph reads (values copied in when armed)
         self._process_params = None  # device vl2_logits_process_params block the processed graphs read (copied when armed)
         self._process_tables = None  # the ops.logits_process_params tensor whose tables the armed block points into
+        self._record_params = None  # device vl2_score_record_params block the recording graphs read (copied when armed)
         self._armed = None          # the graph decode_graph_begin armed last
         self._decode_read = 0
         self.graph_decode = False
@@ -63,6 +67,7 @@ class DecoderEngine:
         """Forget the captured decode steps: they hold the addresses of the KV cache they were captured on."""
         self._decode_graph = self._decode_graph_sampled = self._decode_bufs = self._armed = None
         self._decode_graph_processed = self._decode_graph_sampled_processed = None
+        self._decode_graphs_recorded = {}
 
     def _prefill_last(self, embeds: torch.Tensor) -> torch.Tensor:
         return self.prefill(embeds, all_logits=False, keep_cache=False, _no_graph=True)[0]
@@ -201,13 +206,17 @@ class DecoderEngine:
 
     # ---- the same step as ONE CUDA graph ---------------------------------------------------------------------
     def _decode_body(self, tok_dev: torch.Tensor, pos_dev: torch.Tensor, stage: torch.Tensor, log=None,
-                     sampler: Optional[torch.Tensor] = None, processor: Optional[torch.Tensor] = None) -> torch.Tensor:
+                     sampler: Optional[torch.Tensor] = None, processor: Optional[torch.Tensor] = None,
+                     recorder: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Single-token step whose position and token live in device memory: embeds *tok_dev, appends K/V at *pos_dev,
         writes argmax(logits) back to tok_dev and increments pos_dev, so one captured graph serves every token.
         `sampler` (a device vl2_sample_params block, needs `log`): the new token is drawn by vl2_sample_token with
         counter *step_dev + 1 instead - the n-th new token of a generate() call uses counter n, token 0 came from the
         prefill.  `processor` (a device vl2_logits_process_params block, needs `log`): vl2_process_logits edits the
-        logits first, with the history _decode_hist[0 .. *step_dev + 1) = new tokens 0 .. n - 1."""
+        logits first, with the history _decode_hist[0 .. *step_dev + 1) = new tokens 0 .. n - 1.  `recorder` (a device
+        vl2_score_record_params block, needs `log`): the raw logits row goes to slot n = *step_dev + 1 of its logits
+        buffer before the processors edit it, and the row the token is chosen from (processed; warped by the scored
+        sampler when sampling) to slot n of its scores buffer."""
         Hq, Hkv, D = self.Hq, self.Hkv, self.D
         x = torch.index_select(self.w["embed"], 0, tok_dev)
         o = torch.empty((1, Hq * D), device=x.device, dtype=self.dtype)
@@ -239,12 +248,16 @@ class DecoderEngine:
             h = ops.gemv(x, L["wgu"], act=ops.ACT_SWIGLU, rms_eps=self.eps)
             x = ops.gemv(h, L["wd"], residual=x)
         logits = ops.gemv(x, self.w["lm_head"], rms_eps=self.eps, out_dtype=torch.float32)
+        if recorder is not None:
+            ops.record_rows(logits, recorder, _lib.RECORD_LOGITS, log[1], 1, self.dtype)
         if processor is not None:
             ops.process_logits(logits, processor, self._decode_hist, log[1], 1, self.dtype)
         if sampler is None:
+            if recorder is not None:
+                ops.record_rows(logits, recorder, _lib.RECORD_SCORES, log[1], 1, self.dtype)
             tok_dev.copy_(torch.argmax(logits, dim=1))
         else:
-            ops.sample_token(logits, sampler, log[1], 1, tok_dev, self.dtype)
+            ops.sample_token(logits, sampler, log[1], 1, tok_dev, self.dtype, record=recorder)
         pos_dev.add_(1)
         if log is not None:          # device-side log of the generated ids: the host reads it in chunks, not per token
             gen_buf, step_dev = log
@@ -252,9 +265,11 @@ class DecoderEngine:
             step_dev.add_(1)
         return logits
 
-    def _capture_decode(self, sampler: Optional[torch.Tensor], processor: Optional[torch.Tensor] = None):
+    def _capture_decode(self, sampler: Optional[torch.Tensor], processor: Optional[torch.Tensor] = None,
+                        recorder: Optional[torch.Tensor] = None):
         """Capture the single-token step (greedy, or sampled with the parameter block `sampler`; with the processor
-        block `processor`, the logits processors first) on the shared buffers."""
+        block `processor`, the logits processors first; with the record block `recorder`, recording its rows) on the
+        shared buffers."""
         dev = self.kv[0].device
         if self._decode_bufs is None:
             self._decode_hist = torch.zeros((self.kv[0].shape[0] + 2,), device=dev, dtype=torch.int64)
@@ -274,19 +289,21 @@ class DecoderEngine:
                 pos_dev.fill_(scratch_pos)
                 step_dev.zero_()
                 with ops.pdl(self.decode_pdl):
-                    self._decode_body(tok_dev, pos_dev, stage, log, sampler, processor)
+                    self._decode_body(tok_dev, pos_dev, stage, log, sampler, processor, recorder)
         torch.cuda.current_stream().wait_stream(side)
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph), ops.pdl(self.decode_pdl):
-            logits = self._decode_body(tok_dev, pos_dev, stage, log, sampler, processor)
+            logits = self._decode_body(tok_dev, pos_dev, stage, log, sampler, processor, recorder)
         return (graph, tok_dev, pos_dev, logits, stage)
 
     def decode_graph_begin(self, first_token: int, sampling: Optional[torch.Tensor] = None,
-                           processing: Optional[torch.Tensor] = None) -> None:
+                           processing: Optional[torch.Tensor] = None, recording: Optional[torch.Tensor] = None) -> None:
         """Arm the graph-replayed decode loop after prefill(keep_cache=True): token := first_token, pos := kv_len.
         `sampling`: an ops.sampling_params block - arm the sampled graph (captured once, then reused for every parameter
         setting) instead of the greedy one.  `processing`: an ops.logits_process_params tensor - arm the variant of that
-        graph with the logits processors (also captured once; the tensor is kept alive while armed)."""
+        graph with the logits processors (also captured once; the tensor is kept alive while armed).
+        `recording`: an ops.score_record_params block - arm the recording variant of that graph (captured once per
+        variant): step n writes its rows to slot n of the block's buffers, which must stay alive while armed."""
         if not self.kv:
             raise RuntimeError("decode_graph_begin needs prefill(keep_cache=True) first")
         dev = self.kv[0].device
@@ -297,7 +314,9 @@ class DecoderEngine:
             self._process_params.copy_(processing[:ops.PROCESS_HEADER_WORDS])
             self._process_tables = processing
             proc = self._process_params
-        if sampling is None:
+        if recording is not None:
+            self._arm_recording(recording, sampling, proc)
+        elif sampling is None:
             if proc is None:
                 if self._decode_graph is None:
                     self._decode_graph = self._capture_decode(None)
@@ -324,6 +343,24 @@ class DecoderEngine:
         pos_dev.fill_(self.kv_len)
         self._decode_log[1].zero_()
         self._decode_read = 0
+
+    def _arm_recording(self, recording: torch.Tensor, sampling: Optional[torch.Tensor], proc: Optional[torch.Tensor]):
+        """Arm the recording graph for (sampled, processed), capturing it on first use.  The capture's warm-up steps run
+        with a cleared block, so they write into no caller's buffer."""
+        dev = self.kv[0].device
+        if self._record_params is None or self._record_params.device != dev:
+            self._record_params = torch.zeros((ops.SCORE_RECORD_WORDS,), device=dev, dtype=torch.int64)
+        if sampling is not None:
+            if self._sample_params is None or self._sample_params.device != dev:
+                self._sample_params = torch.zeros((3,), device=dev, dtype=torch.int64)
+            self._sample_params.copy_(sampling)
+        key = (sampling is not None, proc is not None)
+        if key not in self._decode_graphs_recorded:
+            self._record_params.zero_()
+            self._decode_graphs_recorded[key] = self._capture_decode(
+                self._sample_params if sampling is not None else None, proc, self._record_params)
+        self._record_params.copy_(recording)
+        self._armed = self._decode_graphs_recorded[key]
 
     def decode_graph_run(self, k: int) -> None:
         """Enqueue k token steps back to back (no host round trip in between: each replay embeds the token the previous one

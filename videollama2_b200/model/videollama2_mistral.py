@@ -7,7 +7,7 @@ from typing import Dict, List, Optional
 
 import torch
 
-from .. import ops
+from .. import _lib, ops
 from .config import Videollama2Config
 from .videollama2_arch import Videollama2MetaForCausalLM, Videollama2MetaModel
 
@@ -21,6 +21,25 @@ class CausalLMOutput(SimpleNamespace):
 
     def __getitem__(self, i):
         return (self.loss, self.logits)[i] if self.loss is not None else (self.logits,)[i]
+
+
+class GenerateOutput(SimpleNamespace):
+    """Field-compatible with transformers' GenerateDecoderOnlyOutput: what generate(return_dict_in_generate=True)
+    returns.  Attribute access, key access (out["sequences"]) and index access over the fields that are not None."""
+    _FIELDS = ("sequences", "scores", "logits", "attentions", "hidden_states", "past_key_values")
+
+    def __init__(self, sequences, scores=None, logits=None):
+        super().__init__(sequences=sequences, scores=scores, logits=logits, attentions=None, hidden_states=None,
+                         past_key_values=None)
+
+    def keys(self):
+        return [k for k in self._FIELDS if getattr(self, k) is not None]
+
+    def to_tuple(self):
+        return tuple(getattr(self, k) for k in self.keys())
+
+    def __getitem__(self, k):
+        return getattr(self, k) if isinstance(k, str) else self.to_tuple()[k]
 
 
 class EngineKVCache:
@@ -169,7 +188,15 @@ class Videollama2MistralForCausalLM(Videollama2MetaForCausalLM):
         repetition_penalty, no_repeat_ngram_size, min_new_tokens / min_length, bad_words_ids and suppress_tokens, with the
         semantics of transformers 5.5's generate(inputs_embeds=...) - the history is the new tokens only, min_length
         counts the spliced prompt (sampling.generate_processors; the same arithmetic in the reference's pinned 4.40 is
-        unverified).  Without them generation is unchanged."""
+        unverified).  Without them generation is unchanged.
+        return_dict_in_generate=True returns a GenerateOutput (.sequences: the new ids) instead of the id tensor; with
+        output_scores / output_logits its .scores / .logits are tuples of fp32 [B, V] device rows, one per new token, as
+        transformers 5.5's sampling loop records them: `logits` the raw lm_head row, `scores` the row the token was
+        chosen from (after the logits processors, and when sampling after the warpers: l / T where top-k / top-p keep
+        the token, -inf elsewhere).  The rows are recorded on the device on every decode path, inside the decode graphs.
+        Each requested output costs one fp32 [max_new_tokens, V] buffer per call, max_new_tokens * V * 4 bytes (1.25 GB
+        at 2048 tokens and V = 152064, what HF holds too); the tuples are views of its first len(sequences) rows.
+        Without return_dict_in_generate the output_* flags are ignored and nothing is allocated, as in HF."""
         kwargs.pop("position_ids", None)
         attention_mask = kwargs.pop("attention_mask", None)
         if "inputs_embeds" in kwargs:
@@ -178,6 +205,9 @@ class Videollama2MistralForCausalLM(Videollama2MetaForCausalLM):
         temperature = float(kwargs.get("temperature", 1.0) or 1.0)
         top_p, top_k = float(kwargs.get("top_p", 1.0) or 1.0), int(kwargs.get("top_k", 50) or 0)
         rng = kwargs.get("generator")
+        return_dict = bool(kwargs.get("return_dict_in_generate", False))
+        want_scores = return_dict and bool(kwargs.get("output_scores", False))
+        want_logits = return_dict and bool(kwargs.get("output_logits", False))
         if inputs.shape[0] != 1:
             return self._generate_batch(inputs, images, attention_mask, kwargs)
         max_new = int(kwargs.get("max_new_tokens", 20))
@@ -209,14 +239,26 @@ class Videollama2MistralForCausalLM(Videollama2MetaForCausalLM):
             proc = ops.logits_process_params(self.vocab_size, dec.device, **proc)
             history = torch.zeros((max(max_new, 1),), dtype=torch.int64, device=dec.device)
             zero = torch.zeros((1,), dtype=torch.int64, device=dec.device)
+        rec = score_buf = logit_buf = None
+        if want_scores or want_logits:            # row n of each buffer: new token n's row (slot = sampling counter)
+            cap = max(max_new, 0)
+            buf = lambda: torch.empty((cap, self.vocab_size), dtype=torch.float32, device=dec.device)
+            score_buf = buf() if want_scores else None
+            logit_buf = buf() if want_logits else None
+            rec = ops.score_record_params(self.vocab_size, cap, score_buf, logit_buf, dec.device)
+            rec_step = torch.zeros((1,), dtype=torch.int64, device=dec.device)
 
         def pick(logits, n: int) -> int:          # the n-th new token from its logits row
+            if rec is not None:                   # the raw row, before the processors edit it in place
+                ops.record_rows(logits[0], rec, _lib.RECORD_LOGITS, rec_step, n, dec.dtype)
             if proc is not None:                  # processors first, on the ids new tokens 0 .. n - 1
                 ops.process_logits(logits[0], proc, history, zero, n, dec.dtype)
             if params is None:
+                if rec is not None:
+                    ops.record_rows(logits[0], rec, _lib.RECORD_SCORES, rec_step, n, dec.dtype)
                 tok = int(torch.argmax(logits[0]).item())
             else:
-                tok = int(ops.sample_token(logits[0], params, counter, n, tok_out, dec.dtype).item())
+                tok = int(ops.sample_token(logits[0], params, counter, n, tok_out, dec.dtype, record=rec).item())
             if proc is not None and n < max_new:
                 history[n] = tok
             return tok
@@ -226,9 +268,15 @@ class Videollama2MistralForCausalLM(Videollama2MetaForCausalLM):
         use_cache = kwargs.get("use_cache", True)
         self._cache_serial = getattr(self, "_cache_serial", 0) + 1        # handles of earlier forward(use_cache=True) calls die here
         logits, _ = dec.prefill(x, all_logits=False, keep_cache=use_cache and max_new > 1, max_len=S + max_new)
+        def result(ids):
+            if not return_dict:
+                return ids
+            rows = lambda b: None if b is None else tuple(b[i:i + 1] for i in range(ids.shape[1]))
+            return GenerateOutput(ids, rows(score_buf), rows(logit_buf))
+
         if use_cache and max_new > 1 and dec.graph_decode:
-            return self._generate_graphed(dec, pick(logits, 0), max_new, eos_ids, stopping,
-                                          int(kwargs.get("decode_chunk", 8)), params, proc)
+            return result(self._generate_graphed(dec, pick(logits, 0), max_new, eos_ids, stopping,
+                                                 int(kwargs.get("decode_chunk", 8)), params, proc, rec))
         for step in range(max_new):
             tok = pick(logits, step)
             new_ids.append(tok)
@@ -241,7 +289,7 @@ class Videollama2MistralForCausalLM(Videollama2MetaForCausalLM):
             else:   # exact but O(n^2): re-run the prefill kernels on the grown sequence
                 x = torch.cat([x, e], 0)
                 logits, _ = dec.prefill(x, all_logits=False)
-        return torch.tensor([new_ids], dtype=torch.long, device=self.device)
+        return result(torch.tensor([new_ids], dtype=torch.long, device=self.device))
 
     def _generate_batch(self, inputs, images, attention_mask, kwargs):
         """Batch > 1 (HF `generate` semantics of videollama2_mistral.py:110-144 for a padded batch): the rows are decoded
@@ -249,7 +297,9 @@ class Videollama2MistralForCausalLM(Videollama2MetaForCausalLM):
         images its placeholders consume in order (a row without a placeholder consumes one slot, videollama2_arch.py:181-191)
         - and the new ids are right-padded with `pad_token_id` to the longest row, as HF pads finished sequences.  Logits
         processors run per row on that row's new ids; `min_length` counts the row's own spliced length, where HF counts the
-        batch's padded length."""
+        batch's padded length.  With return_dict_in_generate, each output_scores / output_logits step is [B, V]; at the
+        steps after a row stopped, its row is -inf except 0.0 at pad_token_id, so compute_transition_scores gives 0
+        there (HF would decode a pad continuation at those steps, which this engine does not run)."""
         from ..mm_utils import splice_plan
         if kwargs.get("stopping_criteria"):
             raise NotImplementedError("stopping_criteria with batch > 1 (the criteria objects are built for one prompt)")
@@ -268,17 +318,31 @@ class Videollama2MistralForCausalLM(Videollama2MetaForCausalLM):
             mm += used
             out = self.generate(ids.unsqueeze(0), images=imgs, attention_mask=torch.ones((1, ids.numel()), dtype=torch.bool),
                                 **kwargs)
-            rows.append(None if out is None else out[0])
+            rows.append(out)
         if any(r is None for r in rows):       # a frame-parallel rank that does not decode
             return None
-        n = max(int(r.numel()) for r in rows)
+        seqs = [r.sequences[0] if isinstance(r, GenerateOutput) else r[0] for r in rows]
+        n = max(int(r.numel()) for r in seqs)
         res = torch.full((B, n), int(pad), dtype=torch.long, device=self.device)
-        for b, r in enumerate(rows):
+        for b, r in enumerate(seqs):
             res[b, : r.numel()] = r
-        return res
+        if not isinstance(rows[0], GenerateOutput):
+            return res
+
+        def padded(field):                      # [n, B, V]: each row's steps, then the pad row
+            if getattr(rows[0], field) is None:
+                return None
+            out = torch.full((n, B, self.vocab_size), float("-inf"), dtype=torch.float32, device=self.device)
+            out[:, :, int(pad)] = 0.0
+            for b, r in enumerate(rows):
+                steps = getattr(r, field)
+                if steps:
+                    out[:len(steps), b] = torch.cat(steps, 0)
+            return tuple(out.unbind(0))
+        return GenerateOutput(res, padded("scores"), padded("logits"))
 
     def _generate_graphed(self, dec, first: int, max_new: int, eos_ids, stopping, chunk: int, sampling=None,
-                          processing=None):
+                          processing=None, recording=None):
         """Decoding with the host off the critical path: the captured single-token graph feeds itself (token and position
         live in device memory) and appends every new token - the arg-max, or with `sampling` (an ops.sampling_params block)
         the kernel's draw, after the logits processors of `processing` (an ops.logits_process_params tensor) when given -
@@ -295,7 +359,7 @@ class Videollama2MistralForCausalLM(Videollama2MetaForCausalLM):
         ids_buf[0, 0] = first
         n = 1
         if not stops(n):
-            dec.decode_graph_begin(first, sampling, processing)
+            dec.decode_graph_begin(first, sampling, processing, recording)
             done = False
             first = True
             while not done:
@@ -309,6 +373,21 @@ class Videollama2MistralForCausalLM(Videollama2MetaForCausalLM):
                         done = True
                         break
         return ids_buf[:, :n].to(self.device)
+
+    def compute_transition_scores(self, sequences, scores, beam_indices=None, normalize_logits: bool = False):
+        """transformers' compute_transition_scores without beams: [B, steps] fp32, the score of each generated token
+        at its step (log-softmax normalised first when `normalize_logits`), on the scores' device.  `sequences` may
+        hold the prompt in front of the new ids (only its last len(scores) columns are read).  Beam indices raise
+        NotImplementedError: this engine has no beam search."""
+        if beam_indices is not None:
+            raise NotImplementedError("compute_transition_scores: beam search is not supported")
+        steps = len(scores)
+        s = torch.stack(tuple(scores)).reshape(steps, -1).transpose(0, 1)        # [B * V, steps]
+        if normalize_logits:                    # the same reshapes as HF's, so the reduction runs over the same layout
+            s = torch.nn.functional.log_softmax(s.reshape(-1, scores[0].shape[-1], steps), dim=1).reshape(-1, steps)
+        V = scores[0].shape[-1]
+        rows = torch.arange(scores[0].shape[0], device=s.device).view(-1, 1) * V
+        return s.gather(0, sequences[:, sequences.shape[-1] - steps:].to(s.device) + rows)
 
     def prepare_inputs_for_generation(self, input_ids, past_key_values=None, inputs_embeds=None, **kwargs):
         images = kwargs.pop("images", None)

@@ -15,7 +15,7 @@ from ._lib import (ACT_GELU_ERF, ACT_GELU_TANH, ACT_NONE, ACT_QUICK_GELU, ACT_SI
 __all__ = [
     "gemm", "gemm_skinny", "attention", "attention_decode", "decode_rope_append", "attention_decode_dyn", "gemv", "decode_workspace", "l2_prefetch", "layernorm", "rmsnorm", "row_sumsq", "row_stats", "patch_im2col", "patch_embed", "clip_embed_finish",
     "dwconv3x3_ln_silu", "se_scale", "conv3d_im2col", "conv3d_k2s2", "rope_inplace", "embed_splice", "launch_count",
-    "sampling_params", "sample_token", "logits_process_params", "process_logits",
+    "sampling_params", "sample_token", "logits_process_params", "process_logits", "score_record_params", "record_rows",
     "ACT_NONE", "ACT_QUICK_GELU", "ACT_SILU", "ACT_GELU_ERF", "ACT_GELU_TANH", "ACT_SWIGLU", "ACT_SIGMOID",
 ]
 
@@ -366,19 +366,63 @@ def sampling_params(temperature: float, top_k: int, top_p: float, seed: int, dev
 
 
 def sample_token(logits: torch.Tensor, params: torch.Tensor, counter_dev: torch.Tensor, counter_add: int,
-                 out: torch.Tensor, dtype: torch.dtype = torch.bfloat16) -> torch.Tensor:
+                 out: torch.Tensor, dtype: torch.dtype = torch.bfloat16,
+                 record: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Draw one token id from the fp32 logits row [V] (or [1, V]) into out (int64 [1]) with counter *counter_dev +
     counter_add; graph-capturable.  `dtype`: the model's storage type, which picks the library build (the kernel is the
-    same in both)."""
-    _need_cuda(logits, params, counter_dev, out)
+    same in both).  `record` (a score_record_params block): vl2_sample_token_scored also writes the warped row (l / T
+    where kept, -inf elsewhere) to slot *counter_dev + counter_add of the block's scores buffer; the token is the same."""
+    _need_cuda(logits, params, counter_dev, out, record)
     assert logits.dtype == torch.float32 and logits.is_contiguous(), "sample_token: logits are one contiguous fp32 row"
     assert params.dtype == torch.int64 and params.numel() == 3 and params.is_contiguous()
     assert counter_dev.dtype == torch.int64 and counter_dev.numel() == 1
     assert out.dtype == torch.int64 and out.numel() == 1
     lib = _lib.load(dtype)
-    check(lib.vl2_sample_token(logits.data_ptr(), logits.numel(), params.data_ptr(), counter_dev.data_ptr(),
-                               int(counter_add), out.data_ptr(), _stream()), "vl2_sample_token", lib)
+    if record is None:
+        check(lib.vl2_sample_token(logits.data_ptr(), logits.numel(), params.data_ptr(), counter_dev.data_ptr(),
+                                   int(counter_add), out.data_ptr(), _stream()), "vl2_sample_token", lib)
+    else:
+        assert record.dtype == torch.int64 and record.numel() == SCORE_RECORD_WORDS and record.is_contiguous()
+        check(lib.vl2_sample_token_scored(logits.data_ptr(), logits.numel(), params.data_ptr(), counter_dev.data_ptr(),
+                                          int(counter_add), out.data_ptr(), record.data_ptr(), _stream()),
+              "vl2_sample_token_scored", lib)
     return out
+
+
+SCORE_RECORD_WORDS = C.sizeof(_lib.ScoreRecordParams) // 8      # the vl2_score_record_params block, in int64 words
+
+
+def score_record_params(V: int, capacity: int, scores: Optional[torch.Tensor] = None,
+                        logits: Optional[torch.Tensor] = None, device=None) -> torch.Tensor:
+    """The vl2_score_record_params block (int64 [SCORE_RECORD_WORDS], on `device` or the buffers' device) that points
+    record_rows and the scored sampler at `scores` and `logits`, fp32 [capacity, V] buffers (either may be None: nothing
+    is written there).  The block may be copied elsewhere (a captured graph's fixed block) while the buffers stay alive."""
+    V, capacity = int(V), int(capacity)
+    if not 0 < V <= 262144:
+        raise ValueError(f"V = {V} outside [1, 262144]")
+    if capacity < 0:
+        raise ValueError(f"capacity must be >= 0, got {capacity}")
+    for name, t in (("scores", scores), ("logits", logits)):
+        if t is not None and not (t.dtype == torch.float32 and t.is_contiguous() and tuple(t.shape) == (capacity, V)):
+            raise ValueError(f"{name} must be a contiguous fp32 [{capacity}, {V}] tensor, got {t.dtype} {tuple(t.shape)}")
+    if device is None:
+        device = next((t.device for t in (scores, logits) if t is not None), "cpu")
+    p = _lib.ScoreRecordParams(scores=_ptr(scores), logits=_ptr(logits), capacity=capacity, V=V, reserved=0)
+    return torch.frombuffer(bytearray(bytes(p)), dtype=torch.int64).to(device)
+
+
+def record_rows(row: torch.Tensor, params: torch.Tensor, which: int, step_dev: torch.Tensor, add: int,
+                dtype: torch.dtype = torch.bfloat16) -> None:
+    """Copy the fp32 row [V] (or [1, V]) into slot *step_dev + add of the buffer `which` (_lib.RECORD_LOGITS or
+    _lib.RECORD_SCORES) of the score_record_params block `params`; a slot outside [0, capacity) writes nothing.
+    Graph-capturable.  `dtype` picks the library build (the kernel is the same in both)."""
+    _need_cuda(row, params, step_dev)
+    assert row.dtype == torch.float32 and row.is_contiguous(), "record_rows: one contiguous fp32 row"
+    assert params.dtype == torch.int64 and params.numel() == SCORE_RECORD_WORDS and params.is_contiguous()
+    assert step_dev.dtype == torch.int64 and step_dev.numel() == 1
+    lib = _lib.load(dtype)
+    check(lib.vl2_record_row(row.data_ptr(), row.numel(), params.data_ptr(), int(which), step_dev.data_ptr(), int(add),
+                             _stream()), "vl2_record_row", lib)
 
 
 PROCESS_HEADER_WORDS = C.sizeof(_lib.LogitsProcessParams) // 8     # the vl2_logits_process_params block, in int64 words

@@ -7,7 +7,8 @@ computes: `warp_logits` / `sample_token` in plain torch (HF's semantics, any dev
 `kernel_token` / `philox4x32_10`, the kernel's own rule in numpy (fp64), which the tests predict its tokens with.
 
 HF's logits processors (repetition penalty, n-gram and bad-word bans, minimum new tokens, suppressed tokens) run before
-the warpers, on the device in vl2_process_logits (ops.process_logits); `process_logits` here is their host statement."""
+the warpers, on the device in vl2_process_logits (ops.process_logits); `process_logits` here is their host statement.
+`expected_scores` states the row generate(output_scores=True) records for each step."""
 from __future__ import annotations
 
 from typing import Optional
@@ -206,6 +207,18 @@ def kernel_cdf(logits, temperature: float = 1.0, top_k: int = 0, top_p: float = 
 def kernel_token(logits, temperature: float, top_k: int, top_p: float, seed: int, n: int) -> int:
     """The token vl2_sample_token draws with counter n: the first index whose CDF exceeds u."""
     return int(np.searchsorted(kernel_cdf(logits, temperature, top_k, top_p), kernel_u(seed, n), side="right"))
+
+
+def expected_scores(logits: torch.Tensor, history, do_sample: bool = False, temperature: float = 1.0, top_k: int = 0,
+                    top_p: float = 1.0, **processors) -> torch.Tensor:
+    """The `scores` row generate(output_scores=True) records for one raw logits row [V] (a new fp32 CPU row), after the
+    generated ids `history`: process_logits(logits, history, **processors); when sampling, that row's fp32(l / T) where
+    kernel_kept keeps the token and -inf elsewhere - HF's warped row, with the kernel's whole-tie-group top-p rule."""
+    s = process_logits(logits, history, **processors)
+    if not do_sample:
+        return s
+    keep, _ = kernel_kept(s, temperature, top_k, top_p)
+    return torch.where(torch.from_numpy(keep), s / float(temperature), torch.tensor(float("-inf")))
 
 
 def draw_seed(generator: Optional[torch.Generator] = None) -> int:
